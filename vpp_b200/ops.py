@@ -90,7 +90,7 @@ def ingest_rgb_frame(src, border, dst=None, stream=None):
 # ---- stencils -------------------------------------------------------------------------------
 def box5x5_batch(srcs, dsts, stream=None):
     """box5x5 over a batch of (src, dst) pairs in as few launches as possible (vppb_box5x5_*_batch): one persistent launch per
-    32 equally shaped images.  Same results as calling box5x5 pair by pair."""
+    128 equally shaped images.  Same results as calling box5x5 pair by pair."""
     assert len(srcs) == len(dsts) and len(srcs) > 0
     n = len(srcs)
     ins, outs = (capi.VppbImg * n)(), (capi.VppbImg * n)()
