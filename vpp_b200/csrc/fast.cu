@@ -381,7 +381,7 @@ __global__ void __launch_bounds__(256) k_fast9_local_max(Img im, int th, const u
 
 // blockwise maxima (fast.hpp:745-799): per block_size x block_size cell anchored at (0,0), raster
 // scan, strict '>' (first maximum wins), kept iff max > 0.  One thread per cell; bits_out zeroed by caller.
-__global__ void __launch_bounds__(128) k_fast9_block_max(Img im, int th, int bs, const uint32_t* bits, int* cellkp, int wpr,
+__global__ void __launch_bounds__(128) k_fast9_block_max(Img im, int th, int bs, const uint32_t* bits, unsigned* cellkp, int wpr,
                                                         int* rowcount, int cells_r, int cells_c) {
   const long long total = (long long)cells_r * cells_c;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
@@ -405,7 +405,8 @@ __global__ void __launch_bounds__(128) k_fast9_block_max(Img im, int th, int bs,
         c += span;
       }
     }
-    cellkp[i] = vmax > 0 ? ((pr << 16) | pc) : -1;  // one keypoint at most per cell; emitted in CELL raster order
+    // one keypoint at most per cell; emitted in CELL raster order.  Unsigned: rows up to 65535 survive the packing, 0xFFFFFFFF = none
+    cellkp[i] = vmax > 0 ? (((unsigned)pr << 16) | (unsigned)pc) : 0xFFFFFFFFu;
     if (vmax > 0) atomicAdd(&rowcount[(int)(i / cells_c)], 1);
   }
 }
@@ -484,7 +485,7 @@ __global__ void __launch_bounds__(256) k_fast9_emit(Img im, int th, const uint32
 }
 
 // blockwise emit: one warp per row of cells, keypoints leave in cell raster order (the serial order of fast.hpp:763-790)
-__global__ void __launch_bounds__(256) k_fast9_emit_cells(Img im, int th, const int* cellkp, int cells_r, int cells_c, const int* rowoff, vppb_int2* kps,
+__global__ void __launch_bounds__(256) k_fast9_emit_cells(Img im, int th, const unsigned* cellkp, int cells_r, int cells_c, const int* rowoff, vppb_int2* kps,
                                                          int* scores, int capacity) {
   const int lane = threadIdx.x & 31;
   const int warp0 = (int)(((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5);
@@ -494,12 +495,12 @@ __global__ void __launch_bounds__(256) k_fast9_emit_cells(Img im, int th, const 
     if (rowoff[cr + 1] == off) continue;
     for (int c0 = 0; c0 < cells_c; c0 += 32) {
       const int cc = c0 + lane;
-      const int v = cc < cells_c ? cellkp[(long long)cr * cells_c + cc] : -1;
-      const unsigned m = __ballot_sync(0xffffffffu, v >= 0);
-      if (v >= 0) {
+      const unsigned v = cc < cells_c ? cellkp[(long long)cr * cells_c + cc] : 0xFFFFFFFFu;
+      const unsigned m = __ballot_sync(0xffffffffu, v != 0xFFFFFFFFu);
+      if (v != 0xFFFFFFFFu) {
         const int pos = off + __popc(m & ((1u << lane) - 1u));
         if (pos < capacity) {
-          const int r = v >> 16, c = v & 0xFFFF;
+          const int r = (int)(v >> 16), c = (int)(v & 0xFFFFu);
           kps[pos].r = r; kps[pos].c = c;
           if (scores) scores[pos] = (fast9_score_at(im, r, c, th) / 16) & 255;
         }
@@ -514,12 +515,13 @@ __global__ void __launch_bounds__(256) k_fast9_emit_cells(Img im, int th, const 
 // the first slot whose score is smaller -, the table is sorted by decreasing score (stable), slot k of a block is rank k.  One thread
 // per block; the tables go to cellpts / cellsc (maxp entries per block, (row << 16 | col) and raw score), cellcnt = used slots.
 constexpr int FR_MAXP = 16;
-__global__ void __launch_bounds__(128) k_fast9_block_rank(Img im, int th, int bs, int maxp, const uint32_t* bits, int wpr, int* cellpts, int* cellsc,
+__global__ void __launch_bounds__(128) k_fast9_block_rank(Img im, int th, int bs, int maxp, const uint32_t* bits, int wpr, unsigned* cellpts, int* cellsc,
                                                          int* cellcnt, int* rowcount, int cells_r, int cells_c) {
   const long long total = (long long)cells_r * cells_c;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const int r0 = (int)(i / cells_c) * bs, c0 = (int)(i % cells_c) * bs;
-    int pv[FR_MAXP], pp[FR_MAXP];
+    int pv[FR_MAXP];
+    unsigned pp[FR_MAXP];
     for (int k = 0; k < maxp; k++) { pv[k] = 0; pp[k] = 0; }
     for (int r = r0; r < min(r0 + bs, im.nrows); r++) {
       int c = c0;
@@ -543,13 +545,14 @@ __global__ void __launch_bounds__(128) k_fast9_block_rank(Img im, int th, int bs
             }
           if (is_max)
             for (int k = 0; k < maxp; k++)
-              if (pv[k] < v) { pv[k] = v; pp[k] = (r << 16) | cc; break; }
+              if (pv[k] < v) { pv[k] = v; pp[k] = ((unsigned)r << 16) | (unsigned)cc; break; }
         }
         c += span;
       }
     }
     for (int a = 1; a < maxp; a++) {  // std::sort on <= 16 elements == insertion sort: stable
-      const int v = pv[a], q = pp[a];
+      const int v = pv[a];
+      const unsigned q = pp[a];
       int j = a - 1;
       while (j >= 0 && pv[j] < v) { pv[j + 1] = pv[j]; pp[j + 1] = pp[j]; j--; }
       pv[j + 1] = v; pp[j + 1] = q;
@@ -566,7 +569,7 @@ __global__ void __launch_bounds__(128) k_fast9_block_rank(Img im, int th, int bs
 }
 
 // one warp per row of blocks: records (row, col, rank) leave in block raster order, ranks ascending
-__global__ void __launch_bounds__(256) k_fast9_emit_rank(const int* cellpts, const int* cellsc, const int* cellcnt, int cells_r, int cells_c, int maxp,
+__global__ void __launch_bounds__(256) k_fast9_emit_rank(const unsigned* cellpts, const int* cellsc, const int* cellcnt, int cells_r, int cells_c, int maxp,
                                                         const int* rowoff, int* kps3, int* scores, int capacity) {
   const int lane = threadIdx.x & 31;
   const int warp0 = (int)(((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5);
@@ -586,8 +589,8 @@ __global__ void __launch_bounds__(256) k_fast9_emit_rank(const int* cellpts, con
       int pos = off + incl - cnt;
       for (int k = 0; k < cnt; k++, pos++)
         if (pos < capacity) {
-          const int v = cellpts[cell * maxp + k];
-          kps3[3 * pos] = v >> 16; kps3[3 * pos + 1] = v & 0xFFFF; kps3[3 * pos + 2] = k;
+          const unsigned v = cellpts[cell * maxp + k];
+          kps3[3 * pos] = (int)(v >> 16); kps3[3 * pos + 1] = (int)(v & 0xFFFFu); kps3[3 * pos + 2] = k;
           if (scores) scores[pos] = cellsc[cell * maxp + k];
         }
       off += __shfl_sync(0xffffffffu, incl, 31);
@@ -609,7 +612,7 @@ struct FastWs {
   int* rowoff;
   int* bandtotal;
   int* count;   // device copy of the keypoint count of the last call
-  int* cellkp;
+  unsigned* cellkp;
   long long bytes;
 };
 
@@ -626,7 +629,7 @@ static FastWs fast_ws_layout(void* base, int nrows, int ncols, int block_size) {
   w.rowoff = reinterpret_cast<int*>(p + 2 * bits_bytes + rows_bytes);
   w.bandtotal = reinterpret_cast<int*>(p + 2 * bits_bytes + 2 * rows_bytes);   // <= nrows / FB_ROWS + 1 entries fit in rows_bytes
   w.count = reinterpret_cast<int*>(p + 2 * bits_bytes + 3 * rows_bytes);
-  w.cellkp = reinterpret_cast<int*>(p + 2 * bits_bytes + 3 * rows_bytes + 256);
+  w.cellkp = reinterpret_cast<unsigned*>(p + 2 * bits_bytes + 3 * rows_bytes + 256);
   // the cell array only exists for the blockwise mode; block_size <= 0 sizes it for the smallest block the library
   // accepts there (1 pixel), so that a workspace sized without knowing the mode is always large enough
   const int bs = block_size > 0 ? block_size : 1;
@@ -735,8 +738,8 @@ static int fast9_core(const vppb_img* img, int32_t th, const vppb_img* mask, int
       long long blocks = (cells + 127) / 128;
       int grid = (int)(blocks < (long long)sms * 16 ? blocks : (long long)sms * 16);
       if (rank) {
-        int* cellpts = reinterpret_cast<int*>(static_cast<unsigned char*>(workspace) + ws.bytes);
-        int* cellsc = cellpts + cells * rank->maxp;
+        unsigned* cellpts = reinterpret_cast<unsigned*>(static_cast<unsigned char*>(workspace) + ws.bytes);
+        int* cellsc = reinterpret_cast<int*>(cellpts + cells * rank->maxp);
         int* cellcnt = cellsc + cells * rank->maxp;
         k_fast9_block_rank<<<grid, 128, 0, st>>>(im, th, block_size, rank->maxp, ws.bits_a, wpr, cellpts, cellsc, cellcnt, ws.rowcount, cells_r, cells_c);
         k_fast9_scan<<<1, 1024, 0, st>>>(ws.rowcount, ws.rowoff, cells_r);
