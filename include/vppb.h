@@ -193,6 +193,18 @@ int vppb_lbp_u8(const vppb_img* in, const vppb_img* out, void* stream);
 int64_t vppb_local_maxima_filter_workspace_bytes(int32_t nrows, int32_t ncols, int32_t elem_bytes);
 int vppb_local_maxima_filter(const vppb_img* img, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ---- chamfer distance transforms (distance_transforms.hh:86-152) --------------------------------------------------------- */
+/* d4_ / d8_ / d3_4_ / d5_7_11_distance_transform(A, S): the reference's generic_incremental_distance_transform with its four masks
+ * (fill_with_border(S, B = nrows + ncols); S = 0 where A == 0; a forward and a backward raster pass), computed in parallel with the
+ * identical result: every border pixel of `out`, at its whole width (a view's border is its parent's memory), becomes B, and every
+ * domain pixel the mask distance to the nearest zero of `in`, capped at B.  `in`: unsigned char or int pixels compared with 0, its
+ * border is not read; `out`: int, same domain, border >= 1 (>= 2 for d5-7-11: VPPB_E_BORDER), no memory shared with `in` (VPPB_E_ARG).
+ * Pitch padding is never written.  A fixed number of launches per mask, no host synchronisation; `workspace` is device memory of at
+ * least vppb_distance_transform_workspace_bytes bytes, used until the work queued on `stream` completes. */
+enum { VPPB_DT_D4 = 0, VPPB_DT_D8 = 1, VPPB_DT_D3_4 = 2, VPPB_DT_D5_7_11 = 3 };
+int64_t vppb_distance_transform_workspace_bytes(int32_t nrows, int32_t ncols, int32_t kind);
+int vppb_distance_transform(const vppb_img* in, const vppb_img* out, int32_t kind, void* workspace, int64_t workspace_bytes, void* stream);
+
 /* ---- Lucas-Kanade (lucas_kanade.hpp:12-184, lk.hh:42-175, pyrlk_match.hh:15-55) ----------- */
 enum { VPPB_LK_ERR_SAD = 0 /* lucas_kanade.hpp:116-128 */, VPPB_LK_ERR_SAD_OVER_MAD = 1 /* lk.hh:151-173 */ };
 typedef struct vppb_lk_params {

@@ -10,6 +10,7 @@ from .ops import (  # noqa: F401
     Pyramid2d, box5x5, box5x5_batch, clone, copy, copy_with_border, fast9, fast9_scores, fill, fill_border_closest,
     fill_border_mirror, fill_border_with_value, fill_with_border, ingest_rgb_frame, lucas_kanade, pixel_wise_add,
     pyrlk_match, pyrlk_prepare, rgb_to_graylevel, scharr, semi_dense_optical_flow, sum, fast9_blockwise_rank, lbp_transform,
-    local_maxima_filter, oriented_lk_match,
+    local_maxima_filter, oriented_lk_match, d4_distance_transform, d8_distance_transform, d3_4_distance_transform,
+    d5_7_11_distance_transform,
 )
 from . import video_extruder  # noqa: F401,E402

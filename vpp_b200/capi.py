@@ -20,6 +20,7 @@ VPPB_E_NCCL = -5
 FAST_REFERENCE_RING, FAST_TRUE_RING = 0, 1
 FAST_ALL, FAST_LOCAL_MAXIMA, FAST_BLOCKWISE = 0, 1, 2
 LK_ERR_SAD, LK_ERR_SAD_OVER_MAD = 0, 1
+DT_D4, DT_D8, DT_D3_4, DT_D5_7_11 = 0, 1, 2, 3
 
 
 class VppbImg(C.Structure):
@@ -114,6 +115,8 @@ PROTOTYPES = {
     "vppb_lbp_u8": (C.c_int, [_IMG, _IMG, _VP]),
     "vppb_local_maxima_filter_workspace_bytes": (_I64, [_I32, _I32, _I32]),
     "vppb_local_maxima_filter": (C.c_int, [_IMG, _VP, _I64, _VP]),
+    "vppb_distance_transform_workspace_bytes": (_I64, [_I32, _I32, _I32]),
+    "vppb_distance_transform": (C.c_int, [_IMG, _IMG, _I32, _VP, _I64, _VP]),
     "vppb_lk_match_oriented_u8": (C.c_int, [_IMG, _IMG, _IMG, _I32, _I32, C.c_float, _I32, C.c_float, C.c_float, _VP, _VP, _VP, _VP, _I32, _VP, _VP, _VP]),
     "vppb_lk_match_u8": (C.c_int, [_IMG, _IMG, _IMG, _P(VppbLkParams), _VP, _VP, _I32, _VP, _VP, _VP]),
     "vppb_sdof_workspace_bytes": (_I64, [_I32, _I32, _P(VppbSdofParams)]),

@@ -288,6 +288,34 @@ def local_maxima_filter(a, nbh_size=3, stream=None):  # fast.hpp:555-575 (nbh_si
     return a
 
 
+# ---- chamfer distance transforms (distance_transforms.hh:86-152) --------------------------------------------------------
+def _distance_transform(kind, reach, a, b, stream):
+    """b(p) = mask distance from p to the nearest zero of a, capped at B = nrows + ncols; b's whole border becomes B.  a: u8 or
+    i32 (its border is not read); b: i32 of a's domain with a border >= reach, allocated with exactly that border when None."""
+    if b is None:
+        b = Image2d(a.nrows, a.ncols, "i32", border=reach)
+    ws = _DeviceBuffer(lib.vppb_distance_transform_workspace_bytes(a.nrows, a.ncols, kind))
+    check(lib.vppb_distance_transform(a.ptr(), b.ptr(), kind, ws.ptr, ws.nbytes, stream))
+    check(lib.vppb_sync(stream))  # the workspace is released on return
+    return b
+
+
+def d4_distance_transform(a, b=None, stream=None):  # distance_transforms.hh:120-126, 4-neighbourhood, weight 1
+    return _distance_transform(capi.DT_D4, 1, a, b, stream)
+
+
+def d8_distance_transform(a, b=None, stream=None):  # distance_transforms.hh:128-134, 8-neighbourhood, weight 1
+    return _distance_transform(capi.DT_D8, 1, a, b, stream)
+
+
+def d3_4_distance_transform(a, b=None, stream=None):  # distance_transforms.hh:136-142, weights 3 (axes) and 4 (diagonals)
+    return _distance_transform(capi.DT_D3_4, 1, a, b, stream)
+
+
+def d5_7_11_distance_transform(a, b=None, stream=None):  # distance_transforms.hh:144-152, 5x5 with knight moves; border >= 2
+    return _distance_transform(capi.DT_D5_7_11, 2, a, b, stream)
+
+
 # ---- Lucas-Kanade -----------------------------------------------------------------------------
 def oriented_lk_match(a, b, grad, keypoints, prediction, dir1, dir2, winsize, min_ev, max_iterations, convergence_delta, max_step_norm, stream=None):
     """oriented_lk_match_point_square_win<winsize>()(p, tr_prediction, A, B, Ag, min_ev, max_iterations, convergence_delta, max_step_norm,
