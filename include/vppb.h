@@ -237,17 +237,21 @@ int vppb_lk_match_oriented_u8(const vppb_img* a, const vppb_img* b, const vppb_i
 
 /* ---- semi-dense optical flow of video_extruder (semi_dense_optical_flow.hpp:46-214, gradient_descent.hh:10-89) --- */
 typedef struct vppb_sdof_params {
-  int32_t winsize;      /* SAD window side (reference default 7; video_extruder passes 9) */
-  int32_t nscales;      /* pyramid levels (<= 8) */
-  int32_t min_scale;    /* finest level processed */
-  int32_t propagation;  /* number of neighbour-propagation sweeps (even sweeps backward, odd forward) */
-  int32_t patchsize;    /* cell side */
+  int32_t winsize;      /* SAD window side, 1..15 (reference default 7; video_extruder passes 9) */
+  int32_t nscales;      /* pyramid levels, 1..8 */
+  int32_t min_scale;    /* finest level processed, 0..nscales-1 */
+  int32_t propagation;  /* number of neighbour-propagation sweeps per scale, >= 0 (even sweeps backward, odd forward) */
+  int32_t patchsize;    /* cell side, >= 1 */
 } vppb_sdof_params;
 int64_t vppb_sdof_workspace_bytes(int32_t nrows, int32_t ncols, const vppb_sdof_params* params);
 /* pyr1 / pyr2: `nscales` u8 pyramid levels of the two frames (pyramid2d<uchar>(img, nscales, 2, _border >= winsize/2),
  * borders mirror-filled).  kps: n device (row, col) records.  For keypoint i, out_valid[i] tells whether the reference
  * would call match_callback(i, out_pos[i], out_dist[i]).  Serial semantics of the reference: the first keypoint (lowest
- * index) of a cell claims it; propagation sweeps are Gauss-Seidel in the reference's raster orders (wavefront launches). */
+ * index) of a cell claims it; propagation sweeps are Gauss-Seidel in the reference's raster orders.  Schedules: with
+ * propagation <= 30 the whole call is one cooperative launch that solves each sweep by relaxation; above 30, and under
+ * VPPB_SDOF_SCHEDULE=dataflow, one persistent launch per sweep, which takes at most 255 sweeps per scale and
+ * nscales * propagation <= 256 (VPPB_E_ARG otherwise, before anything is launched).  VPPB_SDOF_SCHEDULE=levels and
+ * =antidiagonals take any number of sweeps. */
 int vppb_sdof_u8(const vppb_img* pyr1, const vppb_img* pyr2, const vppb_sdof_params* params, const vppb_int2* kps, int32_t n,
                  void* workspace, int64_t workspace_bytes, vppb_int2* out_pos, int32_t* out_dist, unsigned char* out_valid,
                  void* stream);

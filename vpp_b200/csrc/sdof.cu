@@ -200,9 +200,12 @@ __global__ void k_sdof_clear(SdofLevel L) {
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) { L.mark[i] = 0; L.owner[i] = INT_MAX; L.rec[i] = 0ull; }
 }
 
-__global__ void k_sdof_claim(SdofLevel L, const vppb_int2* kps, int n, int scale_div, int patch) {
+// a keypoint outside the frame (level 0) claims nothing and is reported invalid, also where a coarser level, rounded up, would hold it
+__device__ __forceinline__ bool kp_in_frame(vppb_int2 k, int nrows0, int ncols0) { return k.r >= 0 && k.c >= 0 && k.r < nrows0 && k.c < ncols0; }
+
+__global__ void k_sdof_claim(SdofLevel L, const vppb_int2* kps, int n, int scale_div, int patch, int nrows0, int ncols0) {
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    if (kps[i].r < 0 || kps[i].c < 0) continue;  // a keypoint outside the frame claims nothing (and is reported invalid)
+    if (!kp_in_frame(kps[i], nrows0, ncols0)) continue;
     const int fr = (kps[i].r / scale_div) / patch, fc = (kps[i].c / scale_div) / patch;
     if (fr >= L.cr || fc >= L.cc || kps[i].r / scale_div >= L.i1.nrows || kps[i].c / scale_div >= L.i1.ncols) continue;
     atomicMin(&L.owner[fr * L.cstride + fc], i);
@@ -341,7 +344,7 @@ __global__ void __launch_bounds__(128) k_sdof_prop_wave(SdofLevel L, int t, int 
   }
 }
 
-// ---- dataflow schedule of a sweep (default): ONE persistent launch per sweep ----------------------------------------
+// ---- dataflow schedule of a sweep (propagation > 30, or VPPB_SDOF_SCHEDULE=dataflow): ONE persistent launch per sweep ---
 // Only marked cells do anything in a sweep and a marked cell only reads its marked 8-neighbours, so the Gauss-Seidel order
 // is a partial order on the marked cells: (kr, kc) must come after its marked predecessors (kr, kc-1), (kr-1, kc-1..kc+1)
 // and before its marked successors.  Warps draw iterations from a ticket counter in WAVEFRONT order (anti-diagonal
@@ -389,7 +392,7 @@ __global__ void __launch_bounds__(128) k_sdof_sweep(SdofLevel L, int forward, in
 // k_sdof_levels: ONE CTA walks the anti-diagonals (integer work only, a __syncthreads per diagonal), then buckets the
 // marked cells by level.  sched[0] = number of levels, sched[1] = number of marked cells, start = sched + 2 (cap + 1
 // entries: bucket starts, then the total), hist = start + cap + 1 (scratch: histogram, then bucket cursors).
-// cells: (kr << 16 | kc) of the marked cells, grouped by level (order inside a level is irrelevant: its cells are independent).
+// cells: kr * nkc + kc of the marked cells, grouped by level (order inside a level is irrelevant: its cells are independent).
 __global__ void __launch_bounds__(1024) k_sdof_levels(SdofLevel L, int forward, int nkr, int nkc, int patch, int* level, int* sched, int cap, unsigned* cells) {
   const int inr = L.i1.nrows, inc = L.i1.ncols;
   const int waves = nkc + 2 * (nkr - 1);
@@ -438,17 +441,17 @@ __global__ void __launch_bounds__(1024) k_sdof_levels(SdofLevel L, int forward, 
     const int r = forward ? kr * patch : inr - 1 - kr * patch, c = forward ? kc * patch : inc - 1 - kc * patch;
     const int cell = (r / patch) * L.cstride + (c / patch);
     if (!L.mark[cell]) continue;
-    cells[atomicAdd(&hist[level[cell]], 1)] = ((unsigned)kr << 16) | (unsigned)kc;
+    cells[atomicAdd(&hist[level[cell]], 1)] = (unsigned)i;  // i = kr * nkc + kc: frames may be wider than 65535 cells
   }
 }
 
 // one level of the schedule: n independent iterations, one warp each
-__global__ void __launch_bounds__(128) k_sdof_prop_list(SdofLevel L, const unsigned* cells, int n, int forward, int patch, int ws) {
+__global__ void __launch_bounds__(128) k_sdof_prop_list(SdofLevel L, const unsigned* cells, int n, int forward, int nkc, int patch, int ws) {
   const int lane = threadIdx.x & 31;
   const int nwarps = (gridDim.x * blockDim.x) >> 5;
   for (int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n; i += nwarps) {
-    const unsigned v = cells[i];
-    sdof_prop_cell(L, (int)(v >> 16), (int)(v & 0xFFFFu), forward, patch, ws, lane);
+    const int v = (int)cells[i];
+    sdof_prop_cell(L, v / nkc, v % nkc, forward, patch, ws, lane);
   }
 }
 
@@ -541,7 +544,7 @@ __global__ void __launch_bounds__(256, MINB) k_sdof_fused(const SdofFused P) {
     const int scale_div = 1 << scale;
     for (int i = gtid; i < P.n; i += gthreads) {
       const int kr_ = P.kps[i].r, kc_ = P.kps[i].c;
-      if (kr_ < 0 || kc_ < 0) continue;
+      if (!kp_in_frame(P.kps[i], P.L[0].i1.nrows, P.L[0].i1.ncols)) continue;
       const int fr = (kr_ / scale_div) / P.patch, fc = (kc_ / scale_div) / P.patch;
       if (fr >= L.cr || fc >= L.cc || kr_ / scale_div >= L.i1.nrows || kc_ / scale_div >= L.i1.ncols) continue;
       atomicMin(&L.owner[fr * L.cstride + fc], i);
@@ -602,7 +605,7 @@ __global__ void __launch_bounds__(256, MINB) k_sdof_fused(const SdofFused P) {
     const int kr_ = P.kps[i].r, kc_ = P.kps[i].c;
     const int fr = kr_ / div, fc = kc_ / div;
     int v = 0, pr = 0, pc = 0, d = 0;
-    if (kr_ >= 0 && kc_ >= 0 && fr < L.cr && fc < L.cc && __ldcg(L.mark + fr * L.cstride + fc)) {
+    if (kp_in_frame(P.kps[i], P.L[0].i1.nrows, P.L[0].i1.ncols) && fr < L.cr && fc < L.cc && __ldcg(L.mark + fr * L.cstride + fc)) {
       const unsigned long long rc_ = __ldcg(coarser_rec + fr * L.cstride + fc);
       v = 1; pr = kr_ + rec_fx(rc_) * mul; pc = kc_ + rec_fy(rc_) * mul; d = rec_dist(rc_);
     }
@@ -611,11 +614,12 @@ __global__ void __launch_bounds__(256, MINB) k_sdof_fused(const SdofFused P) {
 }
 
 
-__global__ void k_sdof_emit(SdofLevel L, const vppb_int2* kps, int n, int div, int mul, vppb_int2* pos, int* dist, unsigned char* valid) {
+__global__ void k_sdof_emit(SdofLevel L, const vppb_int2* kps, int n, int div, int mul, int nrows0, int ncols0, vppb_int2* pos, int* dist,
+                            unsigned char* valid) {
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     const int fr = kps[i].r / div, fc = kps[i].c / div;
     int v = 0, pr = 0, pc = 0, d = 0;
-    if (kps[i].r >= 0 && kps[i].c >= 0 && fr < L.cr && fc < L.cc && L.mark[fr * L.cstride + fc]) {
+    if (kp_in_frame(kps[i], nrows0, ncols0) && fr < L.cr && fc < L.cc && L.mark[fr * L.cstride + fc]) {
       const int cell = fr * L.cstride + fc;
       const unsigned long long rc_ = L.rec[cell];
       v = 1; pr = kps[i].r + rec_fx(rc_) * mul; pc = kps[i].c + rec_fy(rc_) * mul; d = rec_dist(rc_);
@@ -689,7 +693,7 @@ int vppb_sdof_u8(const vppb_img* pyr1, const vppb_img* pyr2, const vppb_sdof_par
     w += level_bytes(cr, cc);
   }
   // opt-in: VPPB_SDOF_SCHEDULE=levels runs every sweep as dependency levels of the marked cells when that is shorter than the
-  // anti-diagonals (one blocking read-back of the schedule size per sweep); the default is one launch per anti-diagonal
+  // anti-diagonals (one blocking read-back of the schedule size per sweep), one launch per anti-diagonal otherwise
   const char* sched_env = getenv("VPPB_SDOF_SCHEDULE");
   const bool use_levels = sched_env && strcmp(sched_env, "levels") == 0;
   const bool use_waves = sched_env && strcmp(sched_env, "antidiagonals") == 0;
@@ -703,7 +707,10 @@ int vppb_sdof_u8(const vppb_img* pyr1, const vppb_img* pyr2, const vppb_sdof_par
   unsigned* cell_list = reinterpret_cast<unsigned*>(w + sched_cells * 4);
   int* sched = reinterpret_cast<int*>(w + sched_cells * 8);
   int* tickets = reinterpret_cast<int*>(w + sched_bytes(pyr1[0].nrows, pyr1[0].ncols, p->patchsize) - kCtrBytes);  // 256 counters, one per (scale, sweep)
-  VPPB_REQUIRE(!use_dataflow || p->nscales * p->propagation <= 256, VPPB_E_ARG, "vppb_sdof_u8: more than 256 sweeps");
+  // a dataflow sweep publishes its 1-based number in the record's 8-bit stamp: sweep 256 would read as 0 and its successors
+  // would wait forever; the tickets hold one counter per (scale, sweep)
+  VPPB_REQUIRE(!use_dataflow || (p->propagation <= 255 && p->nscales * p->propagation <= 256), VPPB_E_ARG,
+               "vppb_sdof_u8: the dataflow schedule takes at most 255 sweeps per scale and 256 in all");
   if (use_dataflow) VPPB_CUDA(cudaMemsetAsync(tickets, 0, 1024, st));
   if (use_relax) {
     SdofFused F;
@@ -741,7 +748,7 @@ int vppb_sdof_u8(const vppb_img* pyr1, const vppb_img* pyr2, const vppb_sdof_par
     SdofLevel& Ls = L[scale];
     k_sdof_clear<<<sms * 2, 256, 0, st>>>(Ls);
     if (n > 0) {
-      k_sdof_claim<<<(n + 255) / 256, 256, 0, st>>>(Ls, kps, n, scale_div, p->patchsize);
+      k_sdof_claim<<<(n + 255) / 256, 256, 0, st>>>(Ls, kps, n, scale_div, p->patchsize, pyr1[0].nrows, pyr1[0].ncols);
       const int blocks = (n + 3) / 4;
       k_sdof_match<<<blocks < sms * 16 ? blocks : sms * 16, 128, 0, st>>>(Ls, L[scale + 1 < p->nscales ? scale + 1 : scale], scale < p->nscales - 1 ? 1 : 0, kps,
                                                                         n, scale_div, p->patchsize, p->winsize);
@@ -767,7 +774,7 @@ int vppb_sdof_u8(const vppb_img* pyr1, const vppb_img* pyr2, const vppb_sdof_par
             const int first = h_sched[2 + l], cnt = h_sched[2 + l + 1] - first;
             if (cnt <= 0) continue;
             const int blocks = (cnt + 3) / 4;
-            k_sdof_prop_list<<<blocks < sms * 16 ? blocks : sms * 16, 128, 0, st>>>(Ls, cell_list + first, cnt, forward, p->patchsize, p->winsize);
+            k_sdof_prop_list<<<blocks < sms * 16 ? blocks : sms * 16, 128, 0, st>>>(Ls, cell_list + first, cnt, forward, nkc, p->patchsize, p->winsize);
           }
           continue;
         }
@@ -779,7 +786,9 @@ int vppb_sdof_u8(const vppb_img* pyr1, const vppb_img* pyr2, const vppb_sdof_par
       }
     }
   }
-  if (n > 0) k_sdof_emit<<<(n + 255) / 256, 256, 0, st>>>(L[p->min_scale], kps, n, p->patchsize * (1 << p->min_scale), 1 << p->min_scale, out_pos, out_dist, out_valid);
+  if (n > 0)
+    k_sdof_emit<<<(n + 255) / 256, 256, 0, st>>>(L[p->min_scale], kps, n, p->patchsize * (1 << p->min_scale), 1 << p->min_scale, pyr1[0].nrows, pyr1[0].ncols,
+                                                 out_pos, out_dist, out_valid);
   VPPB_LAUNCH_CHECK("vppb_sdof_u8");
   return VPPB_OK;
 }
