@@ -143,7 +143,11 @@ int vppb_lowpass_sub2_mirror(const vppb_img* in, const vppb_img* out, int kind, 
  * u8 pyramids are built (what semi_dense_optical_flow.hpp:70-100 needs).  Two forms: one launch per step with the three independent
  * chains on three streams forked from / joined into `stream` (default with a gradient pyramid), or ONE cooperative launch - the steps of
  * a level concatenated into a phase of work items, grid-wide barriers between the levels - for images in the library layout (16-byte
- * aligned rows, <= 8 levels; default without a gradient pyramid).  VPPB_PREPARE=fused|streams overrides the choice. */
+ * aligned rows, <= 8 levels; default without a gradient pyramid, which falls back to the streams form when the images or the level count
+ * do not fit it).  VPPB_PREPARE=fused|streams overrides the choice; under `fused` a call that does not fit returns VPPB_E_ARG and says why
+ * (the layout or more than 8 levels).  1 <= nlevels <= 16.  Every step is checked as its stand-alone entry point checks it
+ * (vppb_copy2d_mirror, vppb_scharr_u8_mirror, vppb_lowpass_sub2_mirror) before anything is queued: a call rejected with VPPB_E_ARG or
+ * VPPB_E_BORDER writes nothing. */
 int vppb_pyrlk_prepare(const vppb_img* i1, const vppb_img* i2, const vppb_img* prev, const vppb_img* next, const vppb_img* grad,
                        int32_t nlevels, int32_t grad_is_float, void* stream);
 

@@ -401,16 +401,45 @@ using namespace vppb;
 
 extern "C" {
 
+// ---- argument checks of one step: the stand-alone entry points run them, and vppb_pyrlk_prepare runs those of all its steps before it
+// queues anything.  `who` names the step in the error text.
+static int check_copy_mirror(const vppb_img* src, const vppb_img* dst, const char* who) {  // those of vppb_copy2d_mirror (pixelwise.cu)
+  VPPB_REQUIRE(src && dst && src->base && dst->base, VPPB_E_ARG, "%s: NULL image", who);
+  VPPB_REQUIRE(src->elem_bytes == dst->elem_bytes && src->elem_bytes <= 64, VPPB_E_ARG, "%s: element sizes differ", who);
+  VPPB_REQUIRE(same_domain(src, dst), VPPB_E_ARG, "%s: needs equal domains", who);
+  VPPB_REQUIRE(dst->border <= dst->nrows && dst->border <= dst->ncols, VPPB_E_BORDER, "%s: border %d larger than the image", who, dst->border);
+  return VPPB_OK;
+}
+static int check_scharr(const vppb_img* in, const vppb_img* out, int mirror, const char* who) {
+  VPPB_REQUIRE(in && out && in->base && out->base, VPPB_E_ARG, "%s: NULL image", who);
+  VPPB_REQUIRE(in->elem_bytes == 1 && out->elem_bytes == 8, VPPB_E_ARG, "%s: needs u8 input and 8-byte output elements", who);
+  VPPB_REQUIRE(in->nrows >= out->nrows && in->ncols >= out->ncols, VPPB_E_ARG, "%s: input smaller than output", who);
+  VPPB_REQUIRE(in->border >= 1, VPPB_E_BORDER, "%s: input border %d < 1", who, in->border);
+  VPPB_REQUIRE(((uintptr_t)out->base % 8) == 0 && (out->pitch % 8) == 0, VPPB_E_ARG, "%s: output not 8-byte aligned", who);
+  const int mb = mirror ? out->border : 0;
+  VPPB_REQUIRE(mb <= out->nrows && mb <= out->ncols, VPPB_E_BORDER, "%s: border %d larger than the output image", who, mb);
+  return VPPB_OK;
+}
+static int check_lowpass(const vppb_img* in, const vppb_img* out, int kind, int mirror, const char* who) {
+  VPPB_REQUIRE(in && out && in->base && out->base, VPPB_E_ARG, "%s: NULL image", who);
+  VPPB_REQUIRE(kind >= 0 && kind <= 2, VPPB_E_ARG, "%s: kind %d", who, kind);
+  const int e = kind == 0 ? 1 : 8;
+  VPPB_REQUIRE(in->elem_bytes == e && out->elem_bytes == e, VPPB_E_ARG, "%s: element size must be %d for kind %d", who, e, kind);
+  VPPB_REQUIRE(in->border >= 2, VPPB_E_BORDER, "%s: input border %d < 2", who, in->border);
+  // pyramid.hh:140,154: level size 1 + n/2; any smaller output is a prefix of it
+  VPPB_REQUIRE(out->nrows <= 1 + in->nrows / 2 && out->ncols <= 1 + in->ncols / 2, VPPB_E_ARG,
+               "%s: output %dx%d larger than 1+n/2 of input %dx%d", who, out->nrows, out->ncols, in->nrows, in->ncols);
+  const int mb = mirror ? out->border : 0;
+  VPPB_REQUIRE(mb <= out->nrows && mb <= out->ncols, VPPB_E_BORDER, "%s: border %d larger than the output image", who, mb);
+  return VPPB_OK;
+}
+
 static int scharr_u8(const vppb_img* in, const vppb_img* out, int as_float, int mirror, void* stream) {
-  VPPB_REQUIRE(in && out && in->base && out->base, VPPB_E_ARG, "vppb_scharr_u8: NULL image");
-  VPPB_REQUIRE(in->elem_bytes == 1 && out->elem_bytes == 8, VPPB_E_ARG, "vppb_scharr_u8: needs u8 input and 8-byte output elements");
-  VPPB_REQUIRE(in->nrows >= out->nrows && in->ncols >= out->ncols, VPPB_E_ARG, "vppb_scharr_u8: input smaller than output");
-  VPPB_REQUIRE(in->border >= 1, VPPB_E_BORDER, "vppb_scharr_u8: input border %d < 1", in->border);
-  VPPB_REQUIRE(((uintptr_t)out->base % 8) == 0 && (out->pitch % 8) == 0, VPPB_E_ARG, "vppb_scharr_u8: output not 8-byte aligned");
+  const int rc = check_scharr(in, out, mirror, mirror ? "vppb_scharr_u8_mirror" : "vppb_scharr_u8");
+  if (rc != VPPB_OK) return rc;
   // fast path: 8-byte aligned input rows with >= 4 addressable bytes left of column 0 and enough row to the right
   // of the last group (the library layout pads rows to 128 B), 16-byte aligned output rows
   const int mb = mirror ? out->border : 0;
-  VPPB_REQUIRE(mb <= out->nrows && mb <= out->ncols, VPPB_E_BORDER, "vppb_scharr_u8_mirror: border %d larger than the output image", mb);
   const long long nb = border_items(out->nrows, out->ncols, mb);
   const int groups = (out->ncols + 7) / 8;
   const bool fast = ((uintptr_t)in->base % 8) == 0 && (in->pitch % 8) == 0 && ((uintptr_t)out->base % 16) == 0 && (out->pitch % 16) == 0 &&
@@ -432,16 +461,9 @@ int vppb_scharr_u8(const vppb_img* in, const vppb_img* out, int as_float, void* 
 int vppb_scharr_u8_mirror(const vppb_img* in, const vppb_img* out, int as_float, void* stream) { return scharr_u8(in, out, as_float, 1, stream); }
 
 static int lowpass_sub2(const vppb_img* in, const vppb_img* out, int kind, int mirror, void* stream) {
-  VPPB_REQUIRE(in && out && in->base && out->base, VPPB_E_ARG, "vppb_lowpass_sub2: NULL image");
-  VPPB_REQUIRE(kind >= 0 && kind <= 2, VPPB_E_ARG, "vppb_lowpass_sub2: kind %d", kind);
-  const int e = kind == 0 ? 1 : 8;
-  VPPB_REQUIRE(in->elem_bytes == e && out->elem_bytes == e, VPPB_E_ARG, "vppb_lowpass_sub2: element size must be %d for kind %d", e, kind);
-  VPPB_REQUIRE(in->border >= 2, VPPB_E_BORDER, "vppb_lowpass_sub2: input border %d < 2", in->border);
-  // pyramid.hh:140,154: level size 1 + n/2; any smaller output is a prefix of it
-  VPPB_REQUIRE(out->nrows <= 1 + in->nrows / 2 && out->ncols <= 1 + in->ncols / 2, VPPB_E_ARG,
-               "vppb_lowpass_sub2: output %dx%d larger than 1+n/2 of input %dx%d", out->nrows, out->ncols, in->nrows, in->ncols);
+  const int rc = check_lowpass(in, out, kind, mirror, mirror ? "vppb_lowpass_sub2_mirror" : "vppb_lowpass_sub2");
+  if (rc != VPPB_OK) return rc;
   const int mb = mirror ? out->border : 0;
-  VPPB_REQUIRE(mb <= out->nrows && mb <= out->ncols, VPPB_E_BORDER, "vppb_lowpass_sub2_mirror: border %d larger than the output image", mb);
   cudaStream_t st = as_stream(stream);
   const long long items = (long long)out->nrows * out->ncols * (kind == 0 ? 1 : 2);
   const int grid = grid_for(items, 256);
@@ -533,10 +555,12 @@ static int* prep_barrier_slot() {
   return p + (size_t)(next.fetch_add(1) % 64) * 64;
 }
 
+// *why_not: NULL when the call was queued, else why the images do not fit the fused form (the caller has checked the arguments)
 static int pyrlk_prepare_fused(const vppb_img* i1, const vppb_img* i2, const vppb_img* prev, const vppb_img* next, const vppb_img* grad, int nlevels,
-                               int grad_is_float, cudaStream_t st, bool* done) {
-  *done = false;
+                               int grad_is_float, cudaStream_t st, const char** why_not) {
+  *why_not = "more than 8 levels";
   if (nlevels > PREP_MAX_LEVELS) return VPPB_OK;
+  *why_not = "the images do not have the library layout";
   PrepProg P;
   memset(&P, 0, sizeof(P));
   int n = 0, ph = 0;
@@ -559,6 +583,7 @@ static int pyrlk_prepare_fused(const vppb_img* i1, const vppb_img* i2, const vpp
   P.nphases = ph;
   // the images of one call must be distinct buffers (a phase reads what an earlier phase wrote, never what it writes itself)
   P.bar = prep_barrier_slot();
+  *why_not = "its grid barrier counters could not be allocated";
   if (!P.bar) return VPPB_OK;
   long long most = 0;
   for (int p = 0, first = 0; p < P.nphases; first = P.phase_end[p], p++) {
@@ -573,7 +598,29 @@ static int pyrlk_prepare_fused(const vppb_img* i1, const vppb_img* i2, const vpp
   VPPB_CUDA(cudaMemsetAsync(P.bar, 0, sizeof(int), st));
   VPPB_CUDA(launch_cooperative(k_pyrlk_prepare, (int)blocks, 256, st, P));
   VPPB_LAUNCH_CHECK("vppb_pyrlk_prepare");
-  *done = true;
+  *why_not = nullptr;
+  return VPPB_OK;
+}
+
+// Every check each step of either form makes, in the order of the steps, before anything is queued: a rejected call writes nothing
+// (and leaves no fork of `stream` unjoined).
+static int pyrlk_prepare_check(const vppb_img* i1, const vppb_img* i2, const vppb_img* prev, const vppb_img* next, const vppb_img* grad, int nlevels,
+                               int grad_is_float) {
+  VPPB_REQUIRE(i1 && i2 && prev && next, VPPB_E_ARG, "vppb_pyrlk_prepare: NULL argument");
+  VPPB_REQUIRE(nlevels >= 1 && nlevels <= 16, VPPB_E_ARG, "vppb_pyrlk_prepare: nlevels %d outside 1 .. 16", nlevels);
+  int rc;
+  if ((rc = check_copy_mirror(i1, &prev[0], "vppb_pyrlk_prepare: prev[0] <- i1"))) return rc;
+  if ((rc = check_copy_mirror(i2, &next[0], "vppb_pyrlk_prepare: next[0] <- i2"))) return rc;
+  if (grad && (rc = check_scharr(&prev[0], &grad[0], 1, "vppb_pyrlk_prepare: grad[0] <- scharr(prev[0])"))) return rc;
+  char who[64];
+  for (int l = 1; l < nlevels; l++) {
+    snprintf(who, sizeof(who), "vppb_pyrlk_prepare: prev[%d] <- prev[%d]", l, l - 1);
+    if ((rc = check_lowpass(&prev[l - 1], &prev[l], 0, 1, who))) return rc;
+    snprintf(who, sizeof(who), "vppb_pyrlk_prepare: next[%d] <- next[%d]", l, l - 1);
+    if ((rc = check_lowpass(&next[l - 1], &next[l], 0, 1, who))) return rc;
+    snprintf(who, sizeof(who), "vppb_pyrlk_prepare: grad[%d] <- grad[%d]", l, l - 1);
+    if (grad && (rc = check_lowpass(&grad[l - 1], &grad[l], grad_is_float ? 2 : 1, 1, who))) return rc;
+  }
   return VPPB_OK;
 }
 
@@ -584,7 +631,8 @@ static int pyrlk_prepare_fused(const vppb_img* i1, const vppb_img* i2, const vpp
 // valid inside a stream capture): the critical path is 4 launches instead of 9.
 int vppb_pyrlk_prepare(const vppb_img* i1, const vppb_img* i2, const vppb_img* prev, const vppb_img* next, const vppb_img* grad, int32_t nlevels,
                        int32_t grad_is_float, void* stream) {
-  VPPB_REQUIRE(i1 && i2 && prev && next && nlevels >= 1 && nlevels <= 16, VPPB_E_ARG, "vppb_pyrlk_prepare: bad argument");
+  int rc = pyrlk_prepare_check(i1, i2, prev, next, grad, nlevels, grad_is_float);
+  if (rc != VPPB_OK) return rc;
   {  // Two forms.  "streams": one launch per step, the three independent chains on three streams (forked from / joined into `stream`);
      // "fused": ONE cooperative launch, the steps of a level concatenated into a phase, grid barriers between phases (needs the library
      // layout).  With the gradient pyramid the three concurrent chains are the default (a phase lasts as long as its slowest step, and
@@ -594,10 +642,10 @@ int vppb_pyrlk_prepare(const vppb_img* i1, const vppb_img* i2, const vppb_img* p
     const char* e = getenv("VPPB_PREPARE");
     const bool want_fused = e ? !strcmp(e, "fused") : (grad == nullptr);
     if (want_fused) {
-      bool done = false;
-      const int rc_ = pyrlk_prepare_fused(i1, i2, prev, next, grad, nlevels, grad_is_float, as_stream(stream), &done);
-      if (rc_ != VPPB_OK || done) return rc_;
-      VPPB_REQUIRE(!e, VPPB_E_ARG, "vppb_pyrlk_prepare: VPPB_PREPARE=fused but the images do not have the library layout");
+      const char* why_not = nullptr;
+      rc = pyrlk_prepare_fused(i1, i2, prev, next, grad, nlevels, grad_is_float, as_stream(stream), &why_not);
+      if (rc != VPPB_OK || !why_not) return rc;
+      VPPB_REQUIRE(!e, VPPB_E_ARG, "vppb_pyrlk_prepare: VPPB_PREPARE=fused but %s", why_not);
     }
   }
   static thread_local cudaStream_t side[2] = {nullptr, nullptr};
@@ -612,7 +660,6 @@ int vppb_pyrlk_prepare(const vppb_img* i1, const vppb_img* i2, const vppb_img* p
   }
   cudaStream_t st = as_stream(stream);
   const int gk = grad_is_float ? 2 : 1;
-  int rc;
   // fork: frame 2's pyramid on side[1]
   VPPB_CUDA(cudaEventRecord(ev[0], st));
   VPPB_CUDA(cudaStreamWaitEvent(side[1], ev[0], 0));
