@@ -209,6 +209,39 @@ enum { VPPB_DT_D4 = 0, VPPB_DT_D8 = 1, VPPB_DT_D3_4 = 2, VPPB_DT_D5_7_11 = 3 };
 int64_t vppb_distance_transform_workspace_bytes(int32_t nrows, int32_t ncols, int32_t kind);
 int vppb_distance_transform(const vppb_img* in, const vppb_img* out, int32_t kind, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ---- SAD descriptor matching (descriptor_matcher/*.hh) and patch extraction (core/patch.hh:32-47) ------------------------- */
+/* Descriptors are the rows of an image: `query` and `train` hold one descriptor per row, ncols = its length (>= 1, the same for
+ * both), elem_bytes 1 (unsigned char) or 4 (int, rows 4-byte aligned), any pitch, views included.  The distance is the reference's
+ * sad_distance (distances.hh:9-30), sum |q[k] - t[k]| in int, always summed in full (its early exit only drops candidates that
+ * cannot win); for int descriptors the results are defined when every SAD fits in int32, as in the reference.  index_out and
+ * dist_out are device arrays of query->nrows entries; a query without a candidate gets index -1 and distance INT32_MAX.  Nothing
+ * synchronises the host; `workspace` is device memory of at least the *_workspace_bytes bytes, used until the work queued on
+ * `stream` completes.  Every argument the host can see is checked before anything is queued: a rejected call writes nothing. */
+/* bruteforce_matcher with sad_distance (bruteforce_matcher.hh:11-47): for every query i the train j of smallest SAD, ties to the
+ * lowest j (the reference's strict < scan from j = 0) - index and distance equal the reference's.  Without trains every query
+ * gets (-1, INT32_MAX), where the reference reads train 0 out of bounds.  Workspace: 8 bytes per query, 8-byte aligned. */
+int64_t vppb_match_bruteforce_sad_workspace_bytes(int32_t nquery, int32_t ntrain, int32_t ncols);
+int vppb_match_bruteforce_sad(const vppb_img* query, const vppb_img* train, void* workspace, int64_t workspace_bytes, int32_t* index_out,
+                              int32_t* dist_out, void* stream);
+/* local_index1d_sad_descriptor_matcher (local_index1d_sad_descriptor_matcher.hh:10-57, grid_index.hh:11-88, index1d.hh) at
+ * _approximation = 1: a train's cell is (p.r / s, p.c / s), C division, s = cell_width >= 1; a query's window is the inclusive box
+ * of cells ((q - R) / s, (q + R) / s), R = search_radius >= 0 (whole cells, not a disc of radius R).  The result is the smallest SAD
+ * over the trains of the window's cells, ties to the smallest (cell row, cell col, train index).  The distance always equals the
+ * reference's; the index equals it wherever the reference's choice is determined - inside one cell the reference orders ties by an
+ * unstable std::sort (index1d.hh:41-45).  A train at a coordinate <= -s is never matched (the reference asserts).  Positions are
+ * DEVICE arrays of (row, col).  Workspace (256-byte aligned) depends on ntrain only; the trains are binned by a stable device-side
+ * radix sort on their cell. */
+int64_t vppb_match_local_sad_workspace_bytes(int32_t nquery, int32_t ntrain, int32_t ncols, int32_t search_radius, int32_t cell_width);
+int vppb_match_local_sad(const vppb_img* query, const vppb_img* train, const vppb_int2* query_positions, const vppb_int2* train_positions,
+                         int32_t search_radius, int32_t cell_width, void* workspace, int64_t workspace_bytes, int32_t* index_out,
+                         int32_t* dist_out, void* stream);
+/* extract_patches(kps, img, winsize) (patch.hh:32-47): row k of `out` (n x winsize^2, img's element type) is the winsize x winsize
+ * window centred on keypoints[k] (a DEVICE array), row-major from element 0: element (r + h) * winsize + (c + h) for r, c in
+ * [-h, winsize - h), h = winsize / 2.  Deviation: the reference writes element r * winsize + c, before each row (out of bounds
+ * for keypoint 0); this is the layout it plainly intends.  `img`: unsigned char or int, border >= h (VPPB_E_BORDER); a keypoint
+ * whose window leaves the domain plus border gets a zero row (decided per keypoint on the device). */
+int vppb_extract_patches(const vppb_img* img, const vppb_int2* keypoints, int32_t n, int32_t winsize, const vppb_img* out, void* stream);
+
 /* ---- Lucas-Kanade (lucas_kanade.hpp:12-184, lk.hh:42-175, pyrlk_match.hh:15-55) ----------- */
 enum { VPPB_LK_ERR_SAD = 0 /* lucas_kanade.hpp:116-128 */, VPPB_LK_ERR_SAD_OVER_MAD = 1 /* lk.hh:151-173 */ };
 typedef struct vppb_lk_params {

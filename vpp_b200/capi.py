@@ -117,6 +117,11 @@ PROTOTYPES = {
     "vppb_local_maxima_filter": (C.c_int, [_IMG, _VP, _I64, _VP]),
     "vppb_distance_transform_workspace_bytes": (_I64, [_I32, _I32, _I32]),
     "vppb_distance_transform": (C.c_int, [_IMG, _IMG, _I32, _VP, _I64, _VP]),
+    "vppb_match_bruteforce_sad_workspace_bytes": (_I64, [_I32, _I32, _I32]),
+    "vppb_match_bruteforce_sad": (C.c_int, [_IMG, _IMG, _VP, _I64, _VP, _VP, _VP]),
+    "vppb_match_local_sad_workspace_bytes": (_I64, [_I32, _I32, _I32, _I32, _I32]),
+    "vppb_match_local_sad": (C.c_int, [_IMG, _IMG, _VP, _VP, _I32, _I32, _VP, _I64, _VP, _VP, _VP]),
+    "vppb_extract_patches": (C.c_int, [_IMG, _VP, _I32, _I32, _IMG, _VP]),
     "vppb_lk_match_oriented_u8": (C.c_int, [_IMG, _IMG, _IMG, _I32, _I32, C.c_float, _I32, C.c_float, C.c_float, _VP, _VP, _VP, _VP, _I32, _VP, _VP, _VP]),
     "vppb_lk_match_u8": (C.c_int, [_IMG, _IMG, _IMG, _P(VppbLkParams), _VP, _VP, _I32, _VP, _VP, _VP]),
     "vppb_sdof_workspace_bytes": (_I64, [_I32, _I32, _P(VppbSdofParams)]),

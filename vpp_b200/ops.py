@@ -316,6 +316,80 @@ def d5_7_11_distance_transform(a, b=None, stream=None):  # distance_transforms.h
     return _distance_transform(capi.DT_D5_7_11, 2, a, b, stream)
 
 
+# ---- SAD descriptor matching (descriptor_matcher/*.hh) and patch extraction (patch.hh:32-47) ----------------------------
+_DESC_PIXEL = {np.dtype(np.uint8): "u8", np.dtype(np.int32): "i32"}
+
+
+def _descriptors(d, stream):
+    """(keep-alive, VppbImg) of a descriptor set: an Image2d of u8 or i32 (one descriptor per row), or a 2-D uint8 / int32 array
+    uploaded here; an empty array becomes a descriptor of zero rows"""
+    if isinstance(d, Image2d):
+        return d, d.desc
+    a = np.asarray(d)
+    if a.ndim != 2 or a.dtype not in _DESC_PIXEL:
+        raise TypeError("descriptors: 2-D uint8 or int32 array or Image2d expected, got %s %s" % (a.dtype, a.shape))
+    if a.shape[0] == 0:
+        desc = capi.VppbImg(None, None, 0, a.shape[1], max(1, a.shape[1] * a.itemsize), 0, a.itemsize, 0)
+        return desc, desc
+    img = Image2d(a.shape[0], a.shape[1], _DESC_PIXEL[a.dtype])
+    img.upload(a, stream=stream)
+    return img, img.desc
+
+
+def _positions(p, n, stream):
+    kp = np.ascontiguousarray(p, dtype=np.int32).reshape(-1, 2)
+    if len(kp) != n:
+        raise ValueError("%d positions for %d descriptors" % (len(kp), n))
+    return _DeviceBuffer(kp.nbytes).from_host(kp, stream)
+
+
+def bruteforce_sad_matcher(query, train, stream=None):
+    """bruteforce_matcher(query.nrows, train.nrows, _distance = sad_distance, _match) (bruteforce_matcher.hh:11-47): for every query
+    the train of smallest SAD, ties to the lowest train index.  query / train: Image2d of u8 or i32, or 2-D uint8 / int32 arrays, one
+    descriptor per row.  Returns (index[nq], distance[nq]) int32; (-1, INT32_MAX) for every query when there are no trains."""
+    qk, qd = _descriptors(query, stream)
+    tk, td = _descriptors(train, stream)
+    nq = qd.nrows
+    ws = _DeviceBuffer(lib.vppb_match_bruteforce_sad_workspace_bytes(nq, td.nrows, qd.ncols))
+    d_idx, d_dist = _DeviceBuffer(nq * 4), _DeviceBuffer(nq * 4)
+    check(lib.vppb_match_bruteforce_sad(C.byref(qd), C.byref(td), ws.ptr, ws.nbytes, d_idx.ptr, d_dist.ptr, stream))
+    return d_idx.to_host(np.int32, nq, stream), d_dist.to_host(np.int32, nq, stream)
+
+
+def local_sad_descriptor_matcher(query, train, query_positions, train_positions, search_radius=300, cell_width=300, stream=None):
+    """local_index1d_sad_descriptor_matcher(_query, _train, _query_positions, _train_positions, _search_radius, _cell_width,
+    _distance = sad_distance, _match) (local_index1d_sad_descriptor_matcher.hh:10-57; defaults grid_index.hh:16-17): for every query
+    the train of smallest SAD among the trains whose cell (p / cell_width) lies in the query's window of cells
+    ((q - search_radius) / cell_width .. (q + search_radius) / cell_width), ties to the smallest (cell row, cell col, train index).
+    Positions: (n, 2) int (row, col).  Returns (index[nq], distance[nq]) int32; (-1, INT32_MAX) where the window holds no train."""
+    qk, qd = _descriptors(query, stream)
+    tk, td = _descriptors(train, stream)
+    nq, nt = qd.nrows, td.nrows
+    d_qp, d_tp = _positions(query_positions, nq, stream), _positions(train_positions, nt, stream)
+    ws = _DeviceBuffer(lib.vppb_match_local_sad_workspace_bytes(nq, nt, qd.ncols, search_radius, cell_width))
+    d_idx, d_dist = _DeviceBuffer(nq * 4), _DeviceBuffer(nq * 4)
+    check(lib.vppb_match_local_sad(C.byref(qd), C.byref(td), d_qp.ptr, d_tp.ptr, search_radius, cell_width, ws.ptr, ws.nbytes, d_idx.ptr, d_dist.ptr,
+                                   stream))
+    return d_idx.to_host(np.int32, nq, stream), d_dist.to_host(np.int32, nq, stream)
+
+
+def extract_patches(img, keypoints, winsize, stream=None):
+    """extract_patches(kps, img, winsize) (patch.hh:32-47) with the layout the reference intends: row k of the returned Image2d
+    (len(keypoints) x winsize^2, img's pixel type) is the winsize x winsize window centred on keypoints[k], row-major; a window
+    leaving img's domain plus border gives a zero row.  img: u8 or i32 with border >= winsize / 2."""
+    kp = np.ascontiguousarray(keypoints, dtype=np.int32).reshape(-1, 2)
+    n = len(kp)
+    d_kp = _DeviceBuffer(kp.nbytes).from_host(kp, stream)
+    if n == 0:
+        out = Image2d(0, 0, img.pixel, _desc=capi.VppbImg(None, None, 0, winsize * winsize, max(1, winsize * winsize * img.elem_bytes),
+                                                          0, img.elem_bytes, 0))
+    else:
+        out = Image2d(n, winsize * winsize, img.pixel)
+    check(lib.vppb_extract_patches(img.ptr(), d_kp.ptr, n, winsize, out.ptr(), stream))
+    check(lib.vppb_sync(stream))  # the keypoint buffer is released on return
+    return out
+
+
 # ---- Lucas-Kanade -----------------------------------------------------------------------------
 def oriented_lk_match(a, b, grad, keypoints, prediction, dir1, dir2, winsize, min_ev, max_iterations, convergence_delta, max_step_norm, stream=None):
     """oriented_lk_match_point_square_win<winsize>()(p, tr_prediction, A, B, Ag, min_ev, max_iterations, convergence_delta, max_step_norm,
