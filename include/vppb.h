@@ -293,6 +293,40 @@ int vppb_sdof_u8(const vppb_img* pyr1, const vppb_img* pyr2, const vppb_sdof_par
                  void* workspace, int64_t workspace_bytes, vppb_int2* out_pos, int32_t* out_dist, unsigned char* out_valid,
                  void* stream);
 
+/* ---- sparse optical flow (optical_flow.hh:52-73, optical_flow/sparse_optical_flow.hh:36-112; the reference body never compiled,
+ * so these are this library's semantics, DESIGN §3.9) ------------------------------------------------------------------------------
+ * K1 = fast9(i1, detector_th, _blockwise, _block_size) in its serial order (or the caller's DEVICE keypoints), K2 the same on i2;
+ * D1 / D2 = extract_patches(K1 / K2, winsize) (vppb_extract_patches' layout and zero-row rule); (t, d) = vppb_match_local_sad of D1
+ * (queries at K1) against D2 (trains at K2) with search_radius and cell_width.  One output entry per K1 keypoint: position K1[i],
+ * flow, distance, valid.
+ *   subpixelic = 0: valid where t >= 0 and K1[i] is inside the frame; flow = K2[t] - K1[i], distance = d.
+ *   subpixelic = 1: lucas_kanade(i1, i2, _keypoints = K1, _niterations = lk_iterations, _winsize, _nscales) with the int-truncated
+ *     min_ev / delta and the prediction K2[t] - K1[i] ((0, 0) without a match) divided by 2^nscales; every K1 keypoint inside the frame
+ *     is valid, flow = LK's translation (failure codes (-1,-1) and (0,0) included), distance = SAD in int between row i of D1 and the
+ *     winsize x winsize window of i2 centred on (int)(K1[i] + flow), truncated toward zero; a window leaving i2's domain plus border,
+ *     or a non-finite position, counts as zeros.  winsize odd and 5..15, nscales 1..8 (VPPB_E_ARG).
+ * An entry that is not valid has flow (0, 0) and distance INT32_MAX; a caller keypoint outside i1's domain is never valid.
+ * i1 / i2: unsigned char, same domain (1..65535 per side), borders >= max(3, winsize / 2) read as they are (VPPB_E_BORDER).
+ * keypoints: NULL = detect on i1, else n >= 0 device records.  Outputs: DEVICE arrays of `capacity` entries; *count_out (host) = |K1|;
+ * |K1| > capacity gives VPPB_E_CAPACITY with the count filled in.  Nothing allocates: `workspace` (256-byte aligned, at least
+ * vppb_sparse_flow_workspace_bytes(nrows, ncols, params, keypoints ? n : -1) bytes) holds every intermediate.  Every argument the host
+ * can see is checked before anything is queued: a rejected call writes nothing.  The one host synchronisation is an 8-byte read of
+ * the two keypoint counts after the detections. */
+typedef struct vppb_sof_params {
+  int32_t detector_th;   /* FAST threshold (sparse_optical_flow.hh:46: 5) */
+  int32_t block_size;    /* blockwise FAST cell side >= 1 (:45: 5) */
+  int32_t winsize;       /* patch / LK window side, 1..4096 (:49: 11) */
+  int32_t search_radius; /* matcher radius R >= 0 (the body's _radius: 100) */
+  int32_t cell_width;    /* matcher cell width s >= 1 (grid_index.hh:16: 300) */
+  int32_t subpixelic;    /* 0: integer flows of the matches, 1: Lucas-Kanade refinement */
+  int32_t lk_iterations; /* LK iterations >= 0 (:48: 5) */
+  int32_t nscales;       /* LK pyramid levels 1..8 (lucas_kanade's default 3) */
+} vppb_sof_params;
+int64_t vppb_sparse_flow_workspace_bytes(int32_t nrows, int32_t ncols, const vppb_sof_params* params, int32_t nkeypoints);
+int vppb_sparse_flow_u8(const vppb_img* i1, const vppb_img* i2, const vppb_sof_params* params, const vppb_int2* keypoints, int32_t n,
+                        void* workspace, int64_t workspace_bytes, vppb_int2* pos_out, vppb_float2* flow_out, int32_t* dist_out,
+                        unsigned char* valid_out, int32_t capacity, int32_t* count_out, void* stream);
+
 /* ---- multi-GPU row tiles ------------------------------------------------------------------ */
 /* Pack / unpack the `halo` edge rows of a row tile into/from a contiguous device staging buffer
  * (the payload of the one grouped NCCL neighbour exchange per frame).  which: 0 = top rows

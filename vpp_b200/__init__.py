@@ -12,5 +12,6 @@ from .ops import (  # noqa: F401
     pyrlk_match, pyrlk_prepare, rgb_to_graylevel, scharr, semi_dense_optical_flow, sum, fast9_blockwise_rank, lbp_transform,
     local_maxima_filter, oriented_lk_match, d4_distance_transform, d8_distance_transform, d3_4_distance_transform,
     d5_7_11_distance_transform, bruteforce_sad_matcher, local_sad_descriptor_matcher, extract_patches,
+    sparse_optical_flow,
 )
 from . import video_extruder  # noqa: F401,E402

@@ -66,6 +66,11 @@ class VppbSdofParams(C.Structure):
                 ("patchsize", C.c_int32)]
 
 
+class VppbSofParams(C.Structure):
+    _fields_ = [("detector_th", C.c_int32), ("block_size", C.c_int32), ("winsize", C.c_int32), ("search_radius", C.c_int32),
+                ("cell_width", C.c_int32), ("subpixelic", C.c_int32), ("lk_iterations", C.c_int32), ("nscales", C.c_int32)]
+
+
 _P = C.POINTER
 _IMG = _P(VppbImg)
 _VP = C.c_void_p
@@ -126,6 +131,8 @@ PROTOTYPES = {
     "vppb_lk_match_u8": (C.c_int, [_IMG, _IMG, _IMG, _P(VppbLkParams), _VP, _VP, _I32, _VP, _VP, _VP]),
     "vppb_sdof_workspace_bytes": (_I64, [_I32, _I32, _P(VppbSdofParams)]),
     "vppb_sdof_u8": (C.c_int, [_IMG, _IMG, _P(VppbSdofParams), _VP, _I32, _VP, _I64, _VP, _VP, _VP, _VP]),
+    "vppb_sparse_flow_workspace_bytes": (_I64, [_I32, _I32, _P(VppbSofParams), _I32]),
+    "vppb_sparse_flow_u8": (C.c_int, [_IMG, _IMG, _P(VppbSofParams), _VP, _I32, _VP, _I64, _VP, _VP, _VP, _VP, _I32, _P(_I32), _VP]),
     "vppb_halo_bytes": (_I64, [_IMG, _I32]),
     "vppb_halo_pack": (C.c_int, [_IMG, _I32, C.c_int, _VP, _VP]),
     "vppb_halo_unpack": (C.c_int, [_IMG, _I32, C.c_int, _VP, _VP]),

@@ -794,3 +794,329 @@ int vppb_sdof_u8(const vppb_img* pyr1, const vppb_img* pyr2, const vppb_sdof_par
 }
 
 }  // extern "C"
+
+// ==== sparse optical flow ========================================================================================================
+// FAST keypoints of two frames matched by their patches, optionally refined by Lucas-Kanade.
+// Reference: vpp/algorithms/optical_flow.hh:52-73 (the two declared overloads) and optical_flow/sparse_optical_flow.hh:36-112 (a body
+// the reference keeps under `#if 0`; it never compiled, so the semantics below are this library's, see DESIGN §3.9).
+//
+// One call chains the existing entries on one stream: blockwise FAST on both frames (vppb_fast9_u8_async, one workspace reused),
+// extract_patches on both keypoint sets, the grid-local SAD matcher, and in subpixel mode vppb_pyrlk_prepare + vppb_lk_match_u8.
+// Two kernels of this section fill the gaps: k_sof_seed turns the matches into the integer flow (or LK's keypoints and predictions),
+// k_sof_refine computes the SAD between frame 1's patch and frame 2's window at the refined position.  The only host
+// synchronisation is the 8-byte read of the two keypoint counts after the detections: the patch, matcher and LK entries take
+// their counts on the host.
+// It sits in this file, next to the semi-dense flow, because the CPU emulator builds the library's sources from a fixed list.
+namespace vppb {
+
+constexpr int SOF_WARPS = 8;  // refine: keypoints (warps) per CTA
+
+// One thread per K1 keypoint.  Integer mode: the outputs themselves.  Subpixel mode: position, LK's float keypoint and its prediction
+// (K2[t] - K1[i], or (0, 0) without a match); k_sof_refine writes flow's fate, distance and valid afterwards.
+__global__ void __launch_bounds__(256) k_sof_seed(const vppb_int2* k1, const vppb_int2* k2, const int32_t* idx, const int32_t* dist, int n, int nrows,
+                                                  int ncols, int subpix, vppb_int2* pos, vppb_float2* flow, int32_t* dout, unsigned char* valid,
+                                                  vppb_float2* kf, vppb_float2* pred) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const vppb_int2 p = k1[i];
+  const int t = idx[i];
+  vppb_float2 f;
+  f.r = 0.f;
+  f.c = 0.f;
+  if (t >= 0) {  // 64-bit difference: a caller keypoint may lie anywhere
+    const vppb_int2 q = k2[t];
+    f.r = (float)((long long)q.r - p.r);
+    f.c = (float)((long long)q.c - p.c);
+  }
+  pos[i] = p;
+  if (subpix) {
+    vppb_float2 k;
+    k.r = (float)p.r;
+    k.c = (float)p.c;
+    kf[i] = k;
+    pred[i] = f;
+    return;
+  }
+  const bool ok = t >= 0 && p.r >= 0 && p.r < nrows && p.c >= 0 && p.c < ncols;
+  vppb_float2 z;
+  z.r = 0.f;
+  z.c = 0.f;
+  flow[i] = ok ? f : z;
+  dout[i] = ok ? dist[i] : 0x7fffffff;
+  valid[i] = ok ? 1 : 0;
+}
+
+// One warp per keypoint: SAD in int between row i of D1 and the winsize x winsize window of i2 centred on (int)(K1[i] + flow),
+// truncated toward zero per component (the reference's extract_patch(vfloat2), patch.hh:66-79, in the row-major layout); a window
+// that leaves i2's domain plus border, or a non-finite position, counts as all zeros (extract_patches' zero-row rule).  Lane l
+// takes the 4-element groups l, l + 32, ... of the flattened window: D1's rows are 16-byte aligned, so its group is one word; the
+// window's 4 bytes (consecutive columns of one row of i2, or the end of a row and the start of the next) are gathered, lanes
+// reading consecutive bytes of a row; __vsadu4 sums the group.
+__global__ void __launch_bounds__(32 * SOF_WARPS) k_sof_refine(Img i2, const vppb_int2* k1, Img d1, int n, int ws, vppb_float2* flow, int32_t* dout,
+                                                              unsigned char* valid) {
+  const int k = blockIdx.x * SOF_WARPS + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (k >= n) return;
+  const vppb_int2 p = k1[k];
+  if (!(p.r >= 0 && p.r < i2.nrows && p.c >= 0 && p.c < i2.ncols)) {  // a caller keypoint outside the frame is never valid
+    if (lane == 0) {
+      vppb_float2 z;
+      z.r = 0.f;
+      z.c = 0.f;
+      flow[k] = z;
+      dout[k] = 0x7fffffff;
+      valid[k] = 0;
+    }
+    return;
+  }
+  const vppb_float2 f = flow[k];
+  const float yr = __fadd_rn((float)p.r, f.r), yc = __fadd_rn((float)p.c, f.c);
+  const int h = ws / 2;
+  const long long b = i2.border;
+  // |y| < 2^30: (int) is defined; any window beyond that lies outside every image the entry accepts
+  bool inside = isfinite(yr) && isfinite(yc) && fabsf(yr) < 1073741824.f && fabsf(yc) < 1073741824.f;
+  const int cr = inside ? (int)yr : 0, cc = inside ? (int)yc : 0;
+  inside = inside && (long long)cr - h >= -b && (long long)cr - h + ws - 1 <= i2.nrows - 1 + b && (long long)cc - h >= -b &&
+           (long long)cc - h + ws - 1 <= i2.ncols - 1 + b;
+  const unsigned char* drow = d1.base + (long long)k * d1.pitch;
+  const unsigned char* w0 = i2.base + (long long)(cr - h) * i2.pitch + (cc - h);
+  const int n2 = ws * ws;
+  unsigned s = 0;
+  for (int g = lane; 4 * g < n2; g += 32) {
+    const int e0 = 4 * g;
+    unsigned dw, iw = 0;
+    if (e0 + 3 < n2) {
+      dw = *reinterpret_cast<const unsigned*>(drow + e0);
+    } else {
+      dw = 0;
+      for (int j = 0; e0 + j < n2; j++) dw |= (unsigned)drow[e0 + j] << (8 * j);
+    }
+    if (inside) {
+      int r = e0 / ws, c = e0 - r * ws;
+      for (int j = 0; j < 4 && e0 + j < n2; j++) {
+        iw |= (unsigned)w0[(long long)r * i2.pitch + c] << (8 * j);
+        if (++c == ws) {
+          c = 0;
+          r++;
+        }
+      }
+    }
+    s = __vsadu4(dw, iw) + s;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  if (lane == 0) {
+    dout[k] = (int32_t)s;
+    valid[k] = 1;
+  }
+}
+
+// ---- workspace ----------------------------------------------------------------------------------------------------------------
+static int64_t sof_al(int64_t n) { return (n + 255) & ~(int64_t)255; }
+
+struct SofWs {
+  int32_t* counts;  // [0] = |K1| (detection), [1] = |K2|
+  vppb_int2 *k1, *k2;
+  void* fast;
+  int64_t fast_bytes;
+  unsigned char *d1, *d2;
+  int dpitch;
+  void* match;
+  int64_t match_bytes;
+  int32_t *idx, *dist;
+  vppb_float2 *kf, *pred;
+  float* err;
+  unsigned char* pyr;  // prev, next, grad pyramids: 3 * nscales levels, each sof_al(layout total)
+  int64_t bytes;
+};
+
+static const int SOF_PYR_ALIGN = 128;
+
+static void sof_level_dims(int nrows, int ncols, int l, int& nr, int& nc) {
+  nr = nrows;
+  nc = ncols;
+  for (int k = 0; k < l; k++) {  // pyramid.hh:140,154: 1 + n / 2
+    nr = 1 + nr / 2;
+    nc = 1 + nc / 2;
+  }
+}
+
+static int64_t sof_level_bytes(int nr, int nc, int elem, int border) {
+  int32_t pitch;
+  int64_t total, origin;
+  if (vppb_layout(nr, nc, elem, border, SOF_PYR_ALIGN, &pitch, &total, &origin)) return -1;
+  return sof_al(total);
+}
+
+// Carve the workspace (base may be NULL to size it).  n1 < 0: K1 comes from FAST on i1.
+static SofWs sof_ws(unsigned char* base, int nrows, int ncols, const vppb_sof_params& P, int n1) {
+  SofWs w;
+  const int64_t cells = (int64_t)((nrows + P.block_size - 1) / P.block_size) * ((ncols + P.block_size - 1) / P.block_size);
+  const int64_t c1 = n1 < 0 ? cells : n1, c2 = cells;
+  const int64_t D = (int64_t)P.winsize * P.winsize;
+  int64_t off = 0;
+  auto take = [&](int64_t bytes) {
+    unsigned char* p = base ? base + off : nullptr;
+    off += sof_al(bytes);
+    return p;
+  };
+  w.counts = reinterpret_cast<int32_t*>(take(8));
+  w.k1 = reinterpret_cast<vppb_int2*>(take(n1 < 0 ? c1 * 8 : 0));
+  w.k2 = reinterpret_cast<vppb_int2*>(take(c2 * 8));
+  w.fast_bytes = vppb_fast9_workspace_bytes(nrows, ncols, P.block_size);
+  w.fast = take(w.fast_bytes);
+  w.dpitch = (int)((D + 15) & ~(int64_t)15);
+  w.d1 = take(c1 * w.dpitch);
+  w.d2 = take(c2 * w.dpitch);
+  w.match_bytes = vppb_match_local_sad_workspace_bytes((int32_t)c1, (int32_t)c2, (int32_t)D, P.search_radius, P.cell_width);
+  w.match = take(w.match_bytes);
+  w.idx = reinterpret_cast<int32_t*>(take(c1 * 4));
+  w.dist = reinterpret_cast<int32_t*>(take(c1 * 4));
+  w.kf = w.pred = nullptr;
+  w.err = nullptr;
+  w.pyr = nullptr;
+  if (P.subpixelic) {
+    w.kf = reinterpret_cast<vppb_float2*>(take(c1 * 8));
+    w.pred = reinterpret_cast<vppb_float2*>(take(c1 * 8));
+    w.err = reinterpret_cast<float*>(take(c1 * 4));
+    w.pyr = base ? base + off : nullptr;
+    const int border = P.winsize / 2;
+    for (int l = 0; l < P.nscales; l++) {
+      int nr, nc;
+      sof_level_dims(nrows, ncols, l, nr, nc);
+      off += 2 * sof_level_bytes(nr, nc, 1, border) + sof_level_bytes(nr, nc, 8, border);
+    }
+  }
+  w.bytes = off;
+  return w;
+}
+
+// the argument checks a caller can satisfy: everything but the workspace, the outputs and the keypoint count
+static int sof_check_params(const char* fn, int32_t nrows, int32_t ncols, const vppb_sof_params* P) {
+  VPPB_REQUIRE(P, VPPB_E_ARG, "%s: NULL params", fn);
+  VPPB_REQUIRE(nrows >= 1 && ncols >= 1 && nrows < 65536 && ncols < 65536, VPPB_E_ARG, "%s: image %dx%d outside 1 .. 65535", fn, nrows, ncols);
+  VPPB_REQUIRE(P->block_size >= 1 && P->search_radius >= 0 && P->cell_width >= 1, VPPB_E_ARG,
+               "%s: block_size %d and cell_width %d must be >= 1, search_radius %d >= 0", fn, P->block_size, P->cell_width, P->search_radius);
+  VPPB_REQUIRE(P->winsize >= 1 && P->winsize <= 4096, VPPB_E_ARG, "%s: winsize %d out of [1, 4096]", fn, P->winsize);
+  if (P->subpixelic) {
+    VPPB_REQUIRE(P->winsize >= 5 && P->winsize <= 15 && (P->winsize & 1), VPPB_E_ARG, "%s: with subpixelic, winsize %d must be odd and in 5 .. 15",
+                 fn, P->winsize);
+    VPPB_REQUIRE(P->nscales >= 1 && P->nscales <= 8, VPPB_E_ARG, "%s: nscales %d outside 1 .. 8", fn, P->nscales);
+    VPPB_REQUIRE(P->lk_iterations >= 0, VPPB_E_ARG, "%s: lk_iterations %d < 0", fn, P->lk_iterations);
+  }
+  return VPPB_OK;
+}
+
+}  // namespace vppb
+
+using namespace vppb;
+
+extern "C" {
+
+int64_t vppb_sparse_flow_workspace_bytes(int32_t nrows, int32_t ncols, const vppb_sof_params* params, int32_t nkeypoints) {
+  if (sof_check_params("vppb_sparse_flow_workspace_bytes", nrows, ncols, params)) return 0;
+  return sof_ws(nullptr, nrows, ncols, *params, nkeypoints < 0 ? -1 : nkeypoints).bytes;
+}
+
+int vppb_sparse_flow_u8(const vppb_img* i1, const vppb_img* i2, const vppb_sof_params* params, const vppb_int2* keypoints, int32_t n,
+                        void* workspace, int64_t workspace_bytes, vppb_int2* pos_out, vppb_float2* flow_out, int32_t* dist_out,
+                        unsigned char* valid_out, int32_t capacity, int32_t* count_out, void* stream) {
+  const char* fn = "vppb_sparse_flow_u8";
+  VPPB_REQUIRE(i1 && i2 && i1->base && i2->base && count_out, VPPB_E_ARG, "%s: NULL argument", fn);
+  VPPB_REQUIRE(i1->elem_bytes == 1 && i2->elem_bytes == 1, VPPB_E_ARG, "%s: unsigned char images expected", fn);
+  VPPB_REQUIRE(same_domain(i1, i2), VPPB_E_ARG, "%s: domains %dx%d and %dx%d differ", fn, i1->nrows, i1->ncols, i2->nrows, i2->ncols);
+  int rc = sof_check_params(fn, i1->nrows, i1->ncols, params);
+  if (rc) return rc;
+  const vppb_sof_params P = *params;
+  const int need_border = P.winsize / 2 > 3 ? P.winsize / 2 : 3;
+  VPPB_REQUIRE(i1->border >= need_border && i2->border >= need_border, VPPB_E_BORDER, "%s: borders %d and %d < max(3, winsize / 2) = %d", fn,
+               i1->border, i2->border, need_border);
+  const bool detect = keypoints == nullptr;
+  VPPB_REQUIRE(detect || n >= 0, VPPB_E_ARG, "%s: negative keypoint count %d", fn, n);
+  VPPB_REQUIRE(capacity >= 0 && (capacity == 0 || (pos_out && flow_out && dist_out && valid_out)), VPPB_E_ARG, "%s: NULL output or negative capacity",
+               fn);
+  if (P.subpixelic)  // what vppb_pyrlk_prepare checks of the pyramids built here: a mirror border no larger than any level
+    for (int l = 0; l < P.nscales; l++) {
+      int nr, nc;
+      sof_level_dims(i1->nrows, i1->ncols, l, nr, nc);
+      VPPB_REQUIRE(P.winsize / 2 <= nr && P.winsize / 2 <= nc, VPPB_E_BORDER, "%s: pyramid level %d (%dx%d) smaller than its border %d", fn, l, nr,
+                   nc, P.winsize / 2);
+    }
+  const SofWs need = sof_ws(nullptr, i1->nrows, i1->ncols, P, detect ? -1 : n);
+  VPPB_REQUIRE(workspace && workspace_bytes >= need.bytes && (uintptr_t)workspace % 256 == 0, VPPB_E_ARG,
+               "%s: workspace %lld < %lld bytes (or not 256-byte aligned)", fn, (long long)workspace_bytes, (long long)need.bytes);
+  if (!detect && n > capacity) {
+    *count_out = n;
+    VPPB_REQUIRE(false, VPPB_E_CAPACITY, "%s: %d keypoints exceed the capacity %d", fn, n, capacity);
+  }
+  if (!detect && n == 0) {
+    *count_out = 0;
+    return VPPB_OK;
+  }
+  const SofWs w = sof_ws(static_cast<unsigned char*>(workspace), i1->nrows, i1->ncols, P, detect ? -1 : n);
+  cudaStream_t st = as_stream(stream);
+  const int cells = (int)(((int64_t)(i1->nrows + P.block_size - 1) / P.block_size) * ((i1->ncols + P.block_size - 1) / P.block_size));
+
+  // 1. blockwise FAST on both frames, one workspace; both counts come back in one 8-byte read
+  const vppb_int2* k1 = detect ? w.k1 : keypoints;
+  if (detect && (rc = vppb_fast9_u8_async(i1, P.detector_th, nullptr, VPPB_FAST_BLOCKWISE, P.block_size, VPPB_FAST_REFERENCE_RING, w.fast, w.fast_bytes,
+                                          w.k1, nullptr, cells, w.counts, stream)))
+    return rc;
+  if ((rc = vppb_fast9_u8_async(i2, P.detector_th, nullptr, VPPB_FAST_BLOCKWISE, P.block_size, VPPB_FAST_REFERENCE_RING, w.fast, w.fast_bytes, w.k2,
+                                nullptr, cells, w.counts + 1, stream)))
+    return rc;
+  int32_t counts[2] = {0, 0};
+  VPPB_CUDA(cudaMemcpyAsync(counts, w.counts, sizeof(counts), cudaMemcpyDeviceToHost, st));
+  VPPB_CUDA(cudaStreamSynchronize(st));
+  const int n1 = detect ? counts[0] : n, n2 = counts[1];
+  *count_out = n1;
+  VPPB_REQUIRE(n1 <= capacity, VPPB_E_CAPACITY, "%s: %d keypoints exceed the capacity %d", fn, n1, capacity);
+  if (n1 == 0) return VPPB_OK;
+
+  // 2. patches of both sets: rows of winsize^2 bytes, 16-byte aligned
+  const int D = P.winsize * P.winsize;
+  vppb_img d1 = {w.d1, nullptr, n1, D, w.dpitch, 0, 1, 16};
+  vppb_img d2 = {n2 ? w.d2 : nullptr, nullptr, n2, D, w.dpitch, 0, 1, 16};
+  if ((rc = vppb_extract_patches(i1, k1, n1, P.winsize, &d1, stream))) return rc;
+  if ((rc = vppb_extract_patches(i2, w.k2, n2, P.winsize, &d2, stream))) return rc;
+
+  // 3. grid-local SAD match of frame 1's patches (queries) against frame 2's (trains)
+  if ((rc = vppb_match_local_sad(&d1, &d2, k1, w.k2, P.search_radius, P.cell_width, w.match, w.match_bytes, w.idx, w.dist, stream))) return rc;
+  k_sof_seed<<<(n1 + 255) / 256, 256, 0, st>>>(k1, w.k2, w.idx, w.dist, n1, i1->nrows, i1->ncols, P.subpixelic ? 1 : 0, pos_out, flow_out, dist_out,
+                                               valid_out, w.kf, w.pred);
+  VPPB_LAUNCH_CHECK(fn);
+  if (!P.subpixelic) return VPPB_OK;
+
+  // 4. lucas_kanade(i1, i2, _keypoints = K1, _prediction = integer flow, ...) (lucas_kanade.hpp:135-184), then the SAD at the result
+  vppb_img prev[8], next[8], grad[8];
+  unsigned char* p = w.pyr;
+  const int border = P.winsize / 2;
+  for (int l = 0; l < P.nscales; l++) {
+    int nr, nc;
+    sof_level_dims(i1->nrows, i1->ncols, l, nr, nc);
+    const int64_t b1 = sof_level_bytes(nr, nc, 1, border), b8 = sof_level_bytes(nr, nc, 8, border);
+    if ((rc = vppb_wrap(&prev[l], p, nr, nc, 1, border, SOF_PYR_ALIGN))) return rc;
+    if ((rc = vppb_wrap(&next[l], p + b1, nr, nc, 1, border, SOF_PYR_ALIGN))) return rc;
+    if ((rc = vppb_wrap(&grad[l], p + 2 * b1, nr, nc, 8, border, SOF_PYR_ALIGN))) return rc;
+    p += 2 * b1 + b8;
+  }
+  if ((rc = vppb_pyrlk_prepare(i1, i2, prev, next, grad, P.nscales, 0, stream))) return rc;
+  vppb_lk_params L;
+  L.nlevels = P.nscales;
+  L.min_scale = 0;
+  L.winsize = P.winsize;
+  L.max_iter = P.lk_iterations;
+  L.grad_is_float = 0;
+  L.err_mode = VPPB_LK_ERR_SAD;
+  L.gate_on_max_err = 0;
+  L.min_ev = 0.f;  // lucas_kanade.hpp:143-144 keeps min_ev = 0.0001 and delta = 0.1 in int
+  L.delta = 0.f;
+  L.max_err = 0.f;
+  L.factor = 2.f;
+  L.pred_div = (float)(1 << P.nscales);  // lucas_kanade.hpp:163
+  if ((rc = vppb_lk_match_u8(prev, next, grad, &L, w.kf, w.pred, n1, flow_out, w.err, stream))) return rc;
+  k_sof_refine<<<(n1 + SOF_WARPS - 1) / SOF_WARPS, 32 * SOF_WARPS, 0, st>>>(view(i2), k1, view(&d1), n1, P.winsize, flow_out, dist_out, valid_out);
+  VPPB_LAUNCH_CHECK(fn);
+  return VPPB_OK;
+}
+
+}  // extern "C"

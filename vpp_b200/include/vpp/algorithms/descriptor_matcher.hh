@@ -26,8 +26,6 @@ VPP_DEFINE_SYMBOL(query)
 VPP_DEFINE_SYMBOL(train)
 VPP_DEFINE_SYMBOL(query_positions)
 VPP_DEFINE_SYMBOL(train_positions)
-VPP_DEFINE_SYMBOL(search_radius)
-VPP_DEFINE_SYMBOL(cell_width)
 VPP_DEFINE_SYMBOL(approximation)
 VPP_DEFINE_SYMBOL(distance)
 VPP_DEFINE_SYMBOL(match)

@@ -19,7 +19,6 @@
 namespace vpp {
 
 namespace s {
-VPP_DEFINE_SYMBOL(detector_th)
 VPP_DEFINE_SYMBOL(keypoint_spacing)
 VPP_DEFINE_SYMBOL(detector_period)
 VPP_DEFINE_SYMBOL(max_trajectory_length)

@@ -56,6 +56,10 @@ VPP_DEFINE_SYMBOL(min_ev)
 VPP_DEFINE_SYMBOL(delta)
 VPP_DEFINE_SYMBOL(prediction)
 VPP_DEFINE_SYMBOL(ring)  // extension: _ring = 1 selects the true FAST ring (see include/vppb.h)
+// shared by several algorithm headers (video_extruder, descriptor_matcher, optical_flow), which may be included together
+VPP_DEFINE_SYMBOL(detector_th)
+VPP_DEFINE_SYMBOL(search_radius)
+VPP_DEFINE_SYMBOL(cell_width)
 
 // symbol type of an option or of a bare flag
 template <typename O>

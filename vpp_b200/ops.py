@@ -479,3 +479,38 @@ def semi_dense_optical_flow(keypoints, i1, i2, winsize=7, nscales=4, min_scale=0
                            d_valid.ptr, stream))
     return (d_pos.to_host(np.int32, n * 2, stream).reshape(-1, 2), d_dist.to_host(np.int32, n, stream),
             d_valid.to_host(np.uint8, n, stream).astype(bool))
+
+
+# ---- sparse optical flow ----------------------------------------------------------------------
+_SOF_CACHE = {}  # (nrows, ncols, params, nkeypoints) -> workspace: allocated once per shape, reused
+
+
+def sparse_optical_flow(i1, i2, keypoints=None, detector_th=5, block_size=5, winsize=11, search_radius=100, cell_width=300,
+                        subpixelic=False, lk_iterations=5, nscales=3, stream=None):
+    """sparse_optical_flow(i1, i2, _flow = f, ...) / sparse_optical_flow(keypoints, match_callback, i1, i2, ...)
+    (optical_flow.hh:52-73; defaults sparse_optical_flow.hh:45-49, grid_index.hh:16; semantics DESIGN §3.9): blockwise FAST
+    keypoints K1 of i1 (or `keypoints`, (n, 2) int (row, col)) matched to those of i2 by the grid-local SAD of their winsize x
+    winsize patches, refined by Lucas-Kanade when `subpixelic`.  i1, i2: u8 images of one domain with borders >= max(3, winsize / 2),
+    filled by the caller.  Returns (positions (n, 2) int32 = K1, flow (n, 2) float32, distance (n,) int32, valid (n,) bool): the
+    reference calls its callback for the valid entries, in this order."""
+    P = capi.VppbSofParams(detector_th, block_size, winsize, search_radius, cell_width, 1 if subpixelic else 0, lk_iterations, nscales)
+    d_kp, n = None, -1
+    if keypoints is not None:
+        kp = np.ascontiguousarray(keypoints, dtype=np.int32).reshape(-1, 2)
+        n = len(kp)
+        d_kp = _DeviceBuffer(kp.nbytes).from_host(kp, stream)
+    key = (i1.nrows, i1.ncols, tuple(getattr(P, f) for f, _ in P._fields_), n)
+    ws = _SOF_CACHE.get(key)
+    if ws is None:
+        if len(_SOF_CACHE) > 8:
+            _SOF_CACHE.clear()
+        ws = _SOF_CACHE[key] = _DeviceBuffer(lib.vppb_sparse_flow_workspace_bytes(i1.nrows, i1.ncols, C.byref(P), n))
+    bs = max(1, block_size)
+    cap = n if n >= 0 else ((i1.nrows + bs - 1) // bs) * ((i1.ncols + bs - 1) // bs)
+    d_pos, d_flow, d_dist, d_valid = _DeviceBuffer(cap * 8), _DeviceBuffer(cap * 8), _DeviceBuffer(cap * 4), _DeviceBuffer(cap)
+    count = C.c_int32(0)
+    check(lib.vppb_sparse_flow_u8(i1.ptr(), i2.ptr(), C.byref(P), d_kp.ptr if d_kp else None, max(n, 0), ws.ptr, ws.nbytes, d_pos.ptr, d_flow.ptr,
+                                  d_dist.ptr, d_valid.ptr, cap, C.byref(count), stream))
+    m = count.value
+    return (d_pos.to_host(np.int32, m * 2, stream).reshape(-1, 2), d_flow.to_host(np.float32, m * 2, stream).reshape(-1, 2),
+            d_dist.to_host(np.int32, m, stream), d_valid.to_host(np.uint8, m, stream).astype(bool))
