@@ -237,29 +237,34 @@ __global__ void __launch_bounds__(BX_THREADS, BX_TH == 16 ? 4 : 6) k_box5_bytes_
 }
 
 // ------------------------------------------------------------------ streaming kernel (bytes)
-// A CTA is BS_CWARPS = 4 consumer warps and one producer warp.  A task is a strip of G <= 126 16-byte output groups of one
-// image (one group per consumer lane) over a chunk of R output rows.  A row is cut into strips as equal as whole groups
-// allow: 1080p, 4K and 8K vuchar3 rows are 3, 6 and 12 strips of 120 groups, so no strip ends in a mostly idle warp.
-// Lane 0 of the producer warp walks the CTA's tasks and keeps a ring of BS_STAGES stages in flight, each ONE TMA box of
-// 16 bytes left + 16 G + 16 right by BS_K = 5 rows, shared by all consumer warps.  A stage has a "full" mbarrier (its
-// transaction bytes) and an "empty" one (one arrival per consumer warp done reading it); nothing in the loop waits on a
-// CTA-wide barrier, and the pipeline runs on from one task of the CTA into the next.  Per input row a consumer lane
-//   loads its window from the stage (LDS.64 + LDS.128 + LDS.64: bytes x-8 .. x+23),
+// A task is a band of R output rows of one image across S adjacent strips of its rows (a whole 1080p vuchar3 row; a 4K row is two
+// bands wide, an 8K row four), so a CTA streams nearly contiguous memory: the library pads a 1080p row of 5760 bytes to a 6016-byte
+// pitch.  A strip is G <= 126 16-byte output groups, one per lane of a group of BS_CWARPS consumer warps; a row is cut into strips as
+// equal as whole groups allow (1080p, 4K and 8K vuchar3 rows are 3, 6 and 12 strips of 120 groups), and into bands of as equal
+// strip counts, at most BS_MAX_S.  The CTA is S groups of consumer warps and one producer warp.  Lane 0 of the producer walks the
+// CTA's tasks and keeps a ring of stages in flight; a stage is S TMA boxes (one per strip: 16 bytes left + 16 G + 16 right by
+// BS_K = 5 rows) on one "full" mbarrier, and an "empty" mbarrier takes one arrival per consumer warp done reading it.  Nothing in
+// the loop waits on a CTA-wide barrier, and the pipeline runs on from one task of the CTA into the next.  Per input row a consumer
+// lane
+//   loads its window from its strip's box (LDS.64 + LDS.128 + LDS.64: bytes x-8 .. x+23),
 //   splits the words into packed 16-bit lanes E = (b0,b2), O = (b1,b3) and forms the 5 horizontal taps CS bytes apart
 //     (whole or word-straddling lane pairs, one PRMT each)  ->  H = horizontal 5-sum of the raw row, 8 registers,
 //   slides the vertical window in registers: S += H - H(5 rows ago)  (ring of 5 rows, statically indexed because a
 //     stage is exactly 5 rows),
-//   and for every completed window divides by 25 (exact multiply-shift) and stores its 16 bytes.
+//   and for every completed window divides by 25 (exact multiply-shift) and stores its 16 bytes as one 16-byte store.
 // Horizontal-first means the only data exchanged between lanes is the raw halo, which TMA already put in shared memory.
 constexpr int BS_K = 5;            // rows per stage == rows of the vertical window
 constexpr int BS_MAX_BATCH = 128;  // images per launch (their tensor maps travel in the 32 KB kernel parameter space)
-constexpr int BS_CWARPS = 4;       // consumer warps per CTA; one more warp produces
-constexpr int BS_THREADS = 32 * (BS_CWARPS + 1);
+constexpr int BS_CWARPS = 4;       // consumer warps per strip; one more warp per CTA produces
+constexpr int BS_MAX_S = 3;        // strips per band: 3 x 4 consumer warps + the producer = 416 threads
+constexpr int BS_MAX_THREADS = 32 * (BS_CWARPS * BS_MAX_S + 1);
 constexpr int BS_MAX_G = 126;      // 16-byte groups per strip: a box row of 16 G + 32 bytes stays within TMA's 256 8-byte elements
-constexpr int BS_STAGE_BYTES = BS_K * 2048;  // a multiple of 128 (TMA destination alignment)
-constexpr int BS_STAGES = 6;
-constexpr int BS_CTAS_PER_SM = 3;  // 3 x 6 stages x 10 KB of the H100's 228 KB of shared memory per SM
-constexpr int BS_SMEM = BS_STAGES * BS_STAGE_BYTES + 2 * BS_STAGES * 8;
+constexpr int BS_BOX_BYTES = BS_K * 2048;  // one strip's box of a stage; a multiple of 128 (TMA destination alignment)
+// per band width S = 1, 2, 3: CTAs resident per SM (registers: <= 96 per thread, -Xptxas -v) and stages in each CTA's ring, so that
+// the rings fill about the same 180 - 200 KB of the H100's 228 KB of shared memory per SM
+constexpr int BS_CTAS_PER_SM[BS_MAX_S + 1] = {0, 3, 2, 1};
+constexpr int BS_STAGES[BS_MAX_S + 1] = {0, 6, 5, 6};
+inline int bs_smem(int S) { return BS_STAGES[S] * S * BS_BOX_BYTES + 2 * BS_STAGES[S] * 8; }
 
 template <int NB>
 struct BoxStream {
@@ -271,91 +276,100 @@ struct BoxStream {
   const unsigned char* up_base[NB];
   const unsigned char* dn_base[NB];
   int nimg, out_pitch, nrows, rowbytes, strips, G, boxw, chunks, R, groups, vec_store, total;
+  int S, bands, stages;     // strips per band, bands per row, stages in the ring
   int in_pitch, row_room;   // row_room: addressable bytes of a row from pixel (0,0) to the end of its pitch
 };
 
-// A stage that straddles a row-tile seam: row by row, each from the tile that owns it - the halo rows come straight from
-// the neighbour's (peer GPU's) memory as 1-D bulk copies, so the transfer is part of the kernel's own load pipeline.
+// A stage that straddles a row-tile seam: row by row for each strip of the band, each row from the tile that owns it - the halo
+// rows come straight from the neighbour's (peer GPU's) memory as 1-D bulk copies, so the transfer is part of the kernel's own load
+// pipeline.
 template <int NB>
-__device__ __noinline__ void box_stage_from_tiles(const BoxStream<NB>& p, unsigned char* stage, uint64_t* bar, int img, int strip, int ty) {
+__device__ __noinline__ void box_stage_from_tiles(const BoxStream<NB>& p, unsigned char* stage, uint64_t* bar, int img, int strip0, int nstrips, int ty) {
   const unsigned char* up = p.up_base[img];
   const unsigned char* dn = p.dn_base[img];
-  const int xoff = strip * 16 * p.G - 16;
-  const int len = min(p.boxw, p.row_room - xoff);
-  int rows = 0;
+  int rows = 0, bytes = 0;
   for (int i = 0; i < BS_K; i++) rows += (ty + i - 2 <= p.nrows + 1) ? 1 : 0;
-  mbar_arrive_expect_tx(bar, rows * len);
-  for (int i = 0; i < BS_K; i++) {
-    const int v = ty + i - 2;  // image row of the tile
-    if (v > p.nrows + 1) continue;
-    const unsigned char* src = (v < 0 && up) ? up + (long long)(p.nrows + v) * p.in_pitch
-                             : (v >= p.nrows && dn) ? dn + (long long)(v - p.nrows) * p.in_pitch
-                                                    : p.in_base[img] + (long long)v * p.in_pitch;
-    tma_load_1d(stage + i * p.boxw, src + xoff, len, bar);
+  for (int s = 0; s < nstrips; s++) bytes += rows * min(p.boxw, p.row_room - ((strip0 + s) * 16 * p.G - 16));
+  mbar_arrive_expect_tx(bar, bytes);
+  for (int s = 0; s < nstrips; s++) {
+    const int xoff = (strip0 + s) * 16 * p.G - 16;
+    const int len = min(p.boxw, p.row_room - xoff);
+    for (int i = 0; i < BS_K; i++) {
+      const int v = ty + i - 2;  // image row of the tile
+      if (v > p.nrows + 1) continue;
+      const unsigned char* src = (v < 0 && up) ? up + (long long)(p.nrows + v) * p.in_pitch
+                               : (v >= p.nrows && dn) ? dn + (long long)(v - p.nrows) * p.in_pitch
+                                                      : p.in_base[img] + (long long)v * p.in_pitch;
+      tma_load_1d(stage + s * BS_BOX_BYTES + i * p.boxw, src + xoff, len, bar);
+    }
   }
 }
 
-// Ablations for tools/box_bench.py (VPPB_BOX_ABLATE; their outputs are NOT the box filter):
+// Ablations for tools/box_bench.py and tools/box_ceiling.py (VPPB_BOX_ABLATE; their outputs are NOT the box filter):
 //   BOX_COPY:    the same tasks, TMA boxes and stores, the arithmetic replaced by storing each staged row's own bytes;
 //   BOX_COMPUTE: the first ring of stages is fetched once and then re-read for every later stage (no new TMA), and the
 //                results are folded into one word per lane and task instead of being stored row by row.
 enum { BOX_FILTER = 0, BOX_COPY = 1, BOX_COMPUTE = 2 };
 
 template <int CS, int NB, int MODE = BOX_FILTER>
-__global__ void __launch_bounds__(BS_THREADS, BS_CTAS_PER_SM) k_box5_stream(const __grid_constant__ BoxStream<NB> p) {
+__global__ void __launch_bounds__(BS_MAX_THREADS, 1) k_box5_stream(const __grid_constant__ BoxStream<NB> p) {
   extern __shared__ __align__(128) unsigned char smem[];
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + BS_STAGES * BS_STAGE_BYTES);
-  uint64_t* empty = full + BS_STAGES;
+  const int stage_bytes = p.S * BS_BOX_BYTES;
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + p.stages * stage_bytes);
+  uint64_t* empty = full + p.stages;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int per_img = p.strips * p.chunks;
+  const int per_img = p.bands * p.chunks;
 
   grid_launch_dependents();  // the next kernel of the stream may be scheduled while this one drains (it waits before it reads)
   if (threadIdx.x == 0) {
-    for (int s = 0; s < BS_STAGES; s++) {
+    for (int s = 0; s < p.stages; s++) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], BS_CWARPS);
+      mbar_init(&empty[s], BS_CWARPS * p.S);
     }
     fence_barrier_init();
   }
   __syncthreads();           // barrier init visible to every warp
   grid_dependency_wait();    // launched programmatically: everything above overlapped the previous kernel's tail; its writes are visible now
 
-  if (warp == BS_CWARPS) {
-    // producer: a task is decoded once (two divisions), a stage costs a handful of instructions; only stages that straddle
-    // a row-tile seam take the (out-of-line) row-by-row path
+  if (warp == BS_CWARPS * p.S) {
+    // producer: a task is decoded once (two divisions), a stage costs a handful of instructions per strip; only stages that
+    // straddle a row-tile seam take the (out-of-line) row-by-row path
     if (lane != 0) return;
     int slot = 0;
     uint32_t round = 0;  // completed passes over the ring
     for (int task = blockIdx.x; task < p.total; task += gridDim.x) {
       const int img = task / per_img, rem = task - img * per_img;
-      const int chunk = rem / p.strips, strip = rem - chunk * p.strips;
+      const int chunk = rem / p.bands, band = rem - chunk * p.bands;
+      const int strip0 = band * p.S, nstrips = min(p.S, p.strips - strip0);
       int y = chunk * p.R;  // the stage is rows [y, y + 5) of the tensor map = image rows y - 2 .. y + 2
       const bool seam = (p.up_base[img] && y < 2) || (p.dn_base[img] && y + p.groups * BS_K > p.nrows + 2);
       for (int g = 0; g < p.groups; g++, y += BS_K) {
         if (round > 0) mbar_wait(&empty[slot], (round - 1) & 1);  // every consumer warp is done with the slot's previous stage
-        unsigned char* stage = smem + slot * BS_STAGE_BYTES;
+        unsigned char* stage = smem + slot * stage_bytes;
         if (MODE == BOX_COMPUTE && round > 0)
           mbar_arrive(&full[slot]);
         else if (seam && ((p.up_base[img] && y < 2) || (p.dn_base[img] && y + BS_K > p.nrows + 2)))
-          box_stage_from_tiles<NB>(p, stage, &full[slot], img, strip, y);
+          box_stage_from_tiles<NB>(p, stage, &full[slot], img, strip0, nstrips, y);
         else {
-          mbar_arrive_expect_tx(&full[slot], BS_K * p.boxw);
+          mbar_arrive_expect_tx(&full[slot], nstrips * BS_K * p.boxw);
           // tensor origin = 16 bytes left of x = 0 and 2 rows above y = 0; 8-byte elements (x coordinate * 8 is a multiple of 16)
-          tma_load_2d(stage, &p.maps[img], strip * 2 * p.G, y, &full[slot]);
+          for (int s = 0; s < nstrips; s++) tma_load_2d(stage + s * BS_BOX_BYTES, &p.maps[img], (strip0 + s) * 2 * p.G, y, &full[slot]);
         }
-        if (++slot == BS_STAGES) { slot = 0; round++; }
+        if (++slot == p.stages) { slot = 0; round++; }
       }
     }
     return;
   }
 
-  const int cl = warp * 32 + lane;   // this lane's 16-byte group of the strip
+  const int sg = warp / BS_CWARPS;                        // this warp's strip of the band
+  const int cl = (warp - sg * BS_CWARPS) * 32 + lane;     // this lane's 16-byte group of the strip
   const int cr = min(cl, p.G - 1);   // lanes right of the strip read the last group's window and store nothing
   int slot = 0;
   uint32_t parity = 0;
   for (int task = blockIdx.x; task < p.total; task += gridDim.x) {
     const int img = task / per_img, rem = task - img * per_img;
-    const int chunk = rem / p.strips, strip = rem - chunk * p.strips;
+    const int chunk = rem / p.bands, band = rem - chunk * p.bands;
+    const int strip = band * p.S + sg;  // >= p.strips: a strip group of a narrower last band (reads a stale box, stores nothing)
     const int x = strip * 16 * p.G + 16 * cl;
     const int y0 = chunk * p.R, yend = min(y0 + p.R, p.nrows);
     const int nbytes = cl < p.G ? min(16, p.rowbytes - x) : 0;  // <= 0: nothing of this lane's group is in the image
@@ -374,7 +388,7 @@ __global__ void __launch_bounds__(BS_THREADS, BS_CTAS_PER_SM) k_box5_stream(cons
     unsigned char* drow = dst - 5LL * p.out_pitch;  // advanced once per input row: the row its window completes
     for (int g = 0; g < p.groups; g++) {
       mbar_wait(&full[slot], parity);
-      const unsigned char* st = smem + slot * BS_STAGE_BYTES + 16 * cr;
+      const unsigned char* st = smem + slot * stage_bytes + sg * BS_BOX_BYTES + 16 * cr;
 #pragma unroll
       for (int j = 0; j < BS_K; j++) {
         const unsigned char* rp = st + j * p.boxw;
@@ -412,8 +426,8 @@ __global__ void __launch_bounds__(BS_THREADS, BS_CTAS_PER_SM) k_box5_stream(cons
             for (int q = 0; q < 4; q++) ow[q] = MODE == BOX_COPY ? w[2 + q] : box_div_pack(SE[q], SO[q]);
             if (MODE == BOX_COMPUTE) {
               acc ^= ow[0] ^ ow[1] ^ ow[2] ^ ow[3];
-            } else if (vec) {
-              *reinterpret_cast<uint4*>(drow) = make_uint4(ow[0], ow[1], ow[2], ow[3]);
+            } else if (vec) {  // one 16-byte store (a plain uint4 store of this loop is split into 4-byte stores by NVVM)
+              st_stream(reinterpret_cast<int4*>(drow), make_int4((int)ow[0], (int)ow[1], (int)ow[2], (int)ow[3]));
             } else {  // the right edge of the image, or an output without 16-byte alignment: byte stores, statically indexed
 #pragma unroll
               for (int k = 0; k < 16; k++)
@@ -424,7 +438,7 @@ __global__ void __launch_bounds__(BS_THREADS, BS_CTAS_PER_SM) k_box5_stream(cons
       }
       __syncwarp();  // every lane of the warp is done reading the stage
       if (lane == 0) mbar_arrive(&empty[slot]);
-      if (++slot == BS_STAGES) { slot = 0; parity ^= 1; }
+      if (++slot == p.stages) { slot = 0; parity ^= 1; }
     }
     if (MODE == BOX_COMPUTE && vec) *reinterpret_cast<uint32_t*>(dst) = acc;
   }
@@ -461,23 +475,22 @@ static int box_tile_rows(int nrows, int rowbytes) {
   return tiles16 >= 4LL * sm_count() ? 16 : 8;
 }
 
-// Rows per task: R = 5 m - 4 (a task then reads exactly m stages).  Small R = more tasks (parallelism for a single
-// frame) but 4 extra input rows per task; pick the R with the smallest makespan estimate over the resident CTAs, up to
-// one chunk per strip.
-static int box_stream_rows(long long strips_x_imgs, int nrows, int* chunks_out) {
+// Rows per task: R = 5 m - 4 (a task then reads exactly m stages).  Small R = more tasks (parallelism for few frames) but 4 extra
+// input rows per task; pick the R with the smallest makespan estimate over the resident CTAs, up to one band height per image
+// (1080p x 128: one task per image on the H100's 132 resident CTAs).
+static int box_stream_rows(long long bands_x_imgs, int nrows, long long ctas, int* chunks_out) {
   static int forced = -1;
   if (forced < 0) {
     const char* e = getenv("VPPB_BOX_R");
     forced = e ? atoi(e) : 0;
   }
-  const long long ctas = (long long)sm_count() * BS_CTAS_PER_SM;
   const int m_max = std::max(4, (nrows + 4 + BS_K - 1) / BS_K);
   int best_r = 16;
   double best = 1e300;
   for (int m = 4; m <= m_max; m++) {
     const int r = 5 * m - 4;
     if (forced > 0 && r != forced) continue;
-    const long long chunks = (nrows + r - 1) / r, tasks = chunks * strips_x_imgs;
+    const long long chunks = (nrows + r - 1) / r, tasks = chunks * bands_x_imgs;
     const long long waves = (tasks + ctas - 1) / ctas;
     // per task: m stages of 5 rows + ~2 stages of pipeline fill; a wave costs its slowest CTA
     const double cost = (double)waves * (5.0 * m + 2.0);
@@ -496,7 +509,9 @@ static int box5_stream_launch_nb(const vppb_img* ins, const vppb_img* ups, const
   VPPB_CUDA(cudaGetDevice(&dev));
   const unsigned long long bit = 1ULL << (dev & 63);
   if (!(attr_done.load(std::memory_order_acquire) & bit)) {
-    VPPB_CUDA(cudaFuncSetAttribute(k_box5_stream<CS, NB, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, BS_SMEM));
+    int most = 0;
+    for (int s = 1; s <= BS_MAX_S; s++) most = std::max(most, bs_smem(s));
+    VPPB_CUDA(cudaFuncSetAttribute(k_box5_stream<CS, NB, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, most));
     attr_done.fetch_or(bit, std::memory_order_release);
   }
   BoxStream<NB> p;
@@ -509,10 +524,14 @@ static int box5_stream_launch_nb(const vppb_img* ins, const vppb_img* ups, const
   p.strips = (row_groups + BS_MAX_G - 1) / BS_MAX_G;
   p.G = (row_groups + p.strips - 1) / p.strips;
   p.boxw = 16 * p.G + 32;
-  p.R = box_stream_rows((long long)p.strips * n, nrows, &p.chunks);
+  p.bands = (p.strips + BS_MAX_S - 1) / BS_MAX_S;
+  p.S = (p.strips + p.bands - 1) / p.bands;
+  p.stages = BS_STAGES[p.S];
+  const long long resident = (long long)sm_count() * BS_CTAS_PER_SM[p.S];
+  p.R = box_stream_rows((long long)p.bands * n, nrows, resident, &p.chunks);
   p.groups = (p.R + 4 + BS_K - 1) / BS_K;
   p.vec_store = (((uintptr_t)outs[0].base % 16) == 0 && (outs[0].pitch % 16) == 0) ? 1 : 0;
-  p.total = n * p.strips * p.chunks;
+  p.total = n * p.bands * p.chunks;
   const uint64_t width_el = ((uint64_t)rowbytes + 32 + 7) / 8;
   for (int k = 0; k < n; k++) {
     const vppb_img* in = &ins[k];
@@ -531,8 +550,8 @@ static int box5_stream_launch_nb(const vppb_img* ins, const vppb_img* ups, const
     p.in_pitch = ins[0].pitch;
     p.row_room = ins[0].pitch - (int)bs;
   }
-  const int resident = sm_count() * BS_CTAS_PER_SM;
-  VPPB_CUDA(launch_dependent(k_box5_stream<CS, NB, MODE>, p.total < resident ? p.total : resident, BS_THREADS, BS_SMEM, st, p));
+  const int grid = (int)std::min<long long>(p.total, resident);
+  VPPB_CUDA(launch_dependent(k_box5_stream<CS, NB, MODE>, grid, 32 * (BS_CWARPS * p.S + 1), bs_smem(p.S), st, p));
   VPPB_LAUNCH_CHECK(name);
   return VPPB_OK;
 }
