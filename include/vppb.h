@@ -349,6 +349,9 @@ int32_t vppb_kpc_size(void* handle);                       /* entries, dead ones
 const vppb_int2* vppb_kpc_positions(void* handle);         /* DEVICE array of the entries' positions: the keypoints handed to vppb_sdof_u8 */
 /* flow callback of :45-56: entry i moves to new_pos[i] (velocity, age + 1) if valid[i] and inside the frame, is removed if outside */
 int vppb_kpc_flow_update(void* handle, const vppb_int2* new_pos, const unsigned char* valid, int32_t nrows, int32_t ncols, void* stream);
+/* An entry outside the nrows x ncols frame (a caller's detection can put one there) is skipped the way vppb_fast9_scores skips an
+ * out-of-frame keypoint: the merge gives it age 0 and leaves it out of the grid, the score filter gives it age 0 and the mask
+ * gets nothing painted for it. */
 /* :59-84 merge on the keypoint_spacing grid, the older entry of a cell survives */
 int vppb_kpc_merge(void* handle, int32_t nrows, int32_t ncols, int32_t spacing, void* stream);
 /* :87-91 remove entries whose fast9_score(img, th, position) < min_score (3 in the reference); img: u8, border >= 3 */
@@ -356,12 +359,17 @@ int vppb_kpc_score_filter(void* handle, const vppb_img* img, int32_t th, int32_t
 /* :97-109 detector mask: 1 everywhere (border included), 0 in [-spacing, spacing)^2 around every entry; mask: u8, border >= spacing */
 int vppb_kpc_paint_mask(void* handle, const vppb_img* mask, int32_t spacing, void* stream);
 /* :111-118 add(detections) + compact() + sync_attributes(trajectories, keypoint_trajectory(frame_id)); detections / count as
- * vppb_fast9_u8_async leaves them on the device.  Reads the new entry count back (the one host synchronisation of a frame). */
+ * vppb_fast9_u8_async leaves them on the device.  Reads the new entry count back (the one host synchronisation of a frame).
+ * The first min(*det_count_dev, max_detections, capacity - size) detections, in the detector's order, are appended and the rest
+ * are dropped: a full container takes none, a negative count adds none, and no more than max_detections entries are ever read. */
 int vppb_kpc_add_and_compact(void* handle, const vppb_int2* detections, const int32_t* det_count_dev, int32_t max_detections, int32_t frame_id, void* stream);
 /* :122-133 alive entries push their position (oldest dropped beyond max_trajectory_length), dead entries' trajectories die */
 int vppb_kpc_trajectories_update(void* handle, void* stream);
 /* 6 ints per entry into a DEVICE buffer: row, col, age, trajectory start frame, trajectory length, trajectory alive */
 int vppb_kpc_state_table(void* handle, int32_t* table_dev, void* stream);
+/* into DEVICE buffers, either of which may be NULL: size velocities, and size x max_trajectory_length trajectory points
+ * (row, col), newest first, NaN past the trajectory's length */
+int vppb_kpc_history(void* handle, vppb_int2* velocity_dev, vppb_float2* history_dev, void* stream);
 
 /* ---- multi-GPU row tiles, peer memory ----------------------------------------------------- */
 /* Frames shard by contiguous row tiles, one tile per GPU (SURVEY 8e; the reference's only parallelism is OpenMP over

@@ -149,6 +149,7 @@ PROTOTYPES = {
     "vppb_kpc_add_and_compact": (C.c_int, [_VP, _VP, _VP, _I32, _I32, _VP]),
     "vppb_kpc_trajectories_update": (C.c_int, [_VP, _VP]),
     "vppb_kpc_state_table": (C.c_int, [_VP, _VP, _VP]),
+    "vppb_kpc_history": (C.c_int, [_VP, _VP, _VP, _VP]),
     "vppb_box5x5_u8c3_tiles": (C.c_int, [_IMG, _IMG, _IMG, _IMG, _I32, _VP]),
     "vppb_box5x5_u8_tiles": (C.c_int, [_IMG, _IMG, _IMG, _IMG, _I32, _VP]),
     "vppb_ipc_export": (C.c_int, [_IMG, _VP, _P(_I64)]),

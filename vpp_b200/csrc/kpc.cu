@@ -46,6 +46,9 @@ struct Kpc {
 };
 
 __device__ __forceinline__ int c_div(int a, int b) { return a / b; }  // C++ integer division (truncation)
+// An entry outside the frame (only a caller's detection can put one there) is treated like fast9_scores treats an out-of-frame
+// keypoint: the merge and the score filter remove it and the mask gets nothing painted for it, so no kernel indexes past its buffers.
+__device__ __forceinline__ bool in_frame(vppb_int2 p, int nrows, int ncols) { return p.r >= 0 && p.r < nrows && p.c >= 0 && p.c < ncols; }
 
 __global__ void k_kpc_flow(vppb_int2* pos, vppb_int2* vel, int* age, int n, const vppb_int2* newpos, const unsigned char* valid, int nrows, int ncols) {
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
@@ -65,15 +68,18 @@ __global__ void k_kpc_fill_int(int* a, long long n, int v) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) a[i] = v;
 }
 
-__global__ void k_kpc_link(const vppb_int2* pos, int n, int spacing, int stride, int* cell_head, int* next) {
+__global__ void k_kpc_link(const vppb_int2* pos, int n, int nrows, int ncols, int spacing, int stride, int* cell_head, int* next) {
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    if (!in_frame(pos[i], nrows, ncols)) continue;  // left out of the grid
     const int cell = (c_div(pos[i].r, spacing) + 1) * stride + c_div(pos[i].c, spacing) + 1;
     next[i] = atomicExch(&cell_head[cell], i);
   }
 }
 
-__global__ void k_kpc_merge(const vppb_int2* pos, const int* age, int n, int spacing, int stride, const int* cell_head, const int* next, unsigned char* removed) {
+__global__ void k_kpc_merge(const vppb_int2* pos, const int* age, int n, int nrows, int ncols, int spacing, int stride, const int* cell_head, const int* next,
+                            unsigned char* removed) {
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    if (!in_frame(pos[i], nrows, ncols)) { removed[i] = 1; continue; }
     const int cell = (c_div(pos[i].r, spacing) + 1) * stride + c_div(pos[i].c, spacing) + 1;
     const int a = age[i];
     int before_max = INT_MIN;
@@ -97,6 +103,7 @@ __constant__ signed char c_true_ring[16][2] = {{-3, 0}, {-3, 1}, {-2, 2}, {-1, 3
 // fast.hpp:36-77 (true ring), entries with a score under min_score are removed
 __global__ void k_kpc_score_filter(Img im, int th, int min_score, const vppb_int2* pos, int* age, int n) {
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    if (!in_frame(pos[i], im.nrows, im.ncols)) { age[i] = 0; continue; }  // its ring would leave the 3-pixel border
     const unsigned char* p = im.base + (long long)pos[i].r * im.pitch + pos[i].c;
     const int v = *p;
     int sum_inf = 0, sum_sup = 0;
@@ -110,12 +117,14 @@ __global__ void k_kpc_score_filter(Img im, int th, int min_score, const vppb_int
   }
 }
 
-// one warp per entry zeroes its 2s x 2s square of the mask (the mask has a border of s pixels, so no clipping is needed)
+// one warp per entry zeroes its 2s x 2s square of the mask (the mask has a border of s pixels, so an entry inside the frame needs
+// no clipping; one outside paints nothing)
 __global__ void k_kpc_paint(Img mask, const vppb_int2* pos, int n, int s) {
   const int lane = threadIdx.x & 31;
   const int nwarps = (gridDim.x * blockDim.x) >> 5;
   for (int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n; i += nwarps) {
     const int r = pos[i].r, c = pos[i].c;
+    if (!in_frame(pos[i], mask.nrows, mask.ncols)) continue;
     for (int k = lane; k < 4 * s * s; k += 32) {
       const int dr = k / (2 * s) - s, dc = k % (2 * s) - s;
       mask.base[(long long)(r + dr) * mask.pitch + (c + dc)] = 0;
@@ -123,8 +132,11 @@ __global__ void k_kpc_paint(Img mask, const vppb_int2* pos, int n, int s) {
   }
 }
 
-__global__ void k_kpc_add(vppb_int2* pos, vppb_int2* vel, int* age, int n, const vppb_int2* det, const int* det_count, int capacity, int* count) {
-  const int m = min(*det_count, capacity - n);
+// the first min(count, max_detections, capacity - n) detections enter: a detector's count may exceed what it stored (the total it
+// found), and a negative count adds none
+__global__ void k_kpc_add(vppb_int2* pos, vppb_int2* vel, int* age, int n, const vppb_int2* det, const int* det_count, int max_detections, int capacity,
+                          int* count) {
+  const int m = max(0, min(*det_count, min(max_detections, capacity - n)));
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < m; i += gridDim.x * blockDim.x) {
     pos[n + i] = det[i];
     vel[n + i] = vppb_int2{0, 0};
@@ -203,6 +215,19 @@ __global__ void k_kpc_traj(KpcArrays a, int n, int max_traj) {
       a.tlen[i] = min(a.tlen[i] + 1, max_traj);
     } else {
       a.talive[i] = 0;
+    }
+  }
+}
+
+// velocities, and the trajectories newest first with NaN past their length
+__global__ void k_kpc_history(KpcArrays a, int n, int max_traj, vppb_int2* vel, vppb_float2* hist) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    if (vel) vel[i] = a.vel[i];
+    if (hist) {
+      const int len = a.tlen[i], h = a.thead[i];
+      const float nan = __uint_as_float(0x7fc00000u);
+      for (int k = 0; k < max_traj; k++)
+        hist[(long long)i * max_traj + k] = k < len ? a.thist[(long long)i * max_traj + (h + k) % max_traj] : vppb_float2{nan, nan};
     }
   }
 }
@@ -288,8 +313,8 @@ int vppb_kpc_merge(void* handle, int32_t nrows, int32_t ncols, int32_t spacing, 
   }
   cudaStream_t st = as_stream(stream);
   k_kpc_fill_int<<<grid_for(cells), 256, 0, st>>>(k->cell_head, cells, -1);
-  k_kpc_link<<<grid_for(k->n), 256, 0, st>>>(k->pos[k->cur], k->n, spacing, stride, k->cell_head, k->next);
-  k_kpc_merge<<<grid_for(k->n), 256, 0, st>>>(k->pos[k->cur], k->age[k->cur], k->n, spacing, stride, k->cell_head, k->next, k->removed);
+  k_kpc_link<<<grid_for(k->n), 256, 0, st>>>(k->pos[k->cur], k->n, nrows, ncols, spacing, stride, k->cell_head, k->next);
+  k_kpc_merge<<<grid_for(k->n), 256, 0, st>>>(k->pos[k->cur], k->age[k->cur], k->n, nrows, ncols, spacing, stride, k->cell_head, k->next, k->removed);
   k_kpc_apply_removed<<<grid_for(k->n), 256, 0, st>>>(k->age[k->cur], k->removed, k->n);
   VPPB_LAUNCH_CHECK("vppb_kpc_merge");
   return VPPB_OK;
@@ -322,12 +347,12 @@ int vppb_kpc_paint_mask(void* handle, const vppb_img* mask, int32_t spacing, voi
 // append the detections (device array + device count, as vppb_fast9_u8_async leaves them), compact, start trajectories for
 // the newcomers; reads the new entry count back (4 bytes, one synchronisation) because the host sizes later launches with it
 int vppb_kpc_add_and_compact(void* handle, const vppb_int2* detections, const int32_t* det_count_dev, int32_t max_detections, int32_t frame_id, void* stream) {
-  VPPB_REQUIRE(handle && det_count_dev && (detections || max_detections == 0), VPPB_E_ARG, "vppb_kpc_add_and_compact: NULL argument");
+  VPPB_REQUIRE(handle && det_count_dev && max_detections >= 0 && (detections || max_detections == 0), VPPB_E_ARG, "vppb_kpc_add_and_compact: NULL argument");
   Kpc* k = static_cast<Kpc*>(handle);
   cudaStream_t st = as_stream(stream);
   const int cur = k->cur, n_traj = k->n;
   const long long upper = std::min<long long>((long long)k->n + max_detections, k->capacity);
-  k_kpc_add<<<grid_for(std::max(1, max_detections)), 256, 0, st>>>(k->pos[cur], k->vel[cur], k->age[cur], k->n, detections, det_count_dev, k->capacity, k->count);
+  k_kpc_add<<<grid_for(std::max(1, max_detections)), 256, 0, st>>>(k->pos[cur], k->vel[cur], k->age[cur], k->n, detections, det_count_dev, max_detections, k->capacity, k->count);
   k_kpc_scan<<<1, 1024, 0, st>>>(k->age[cur], k->map, k->count);
   k_kpc_gather<<<grid_for(std::max<long long>(1, upper)), 256, 0, st>>>(arrays(k, cur), arrays(k, cur ^ 1), k->map, k->count, n_traj, frame_id, k->max_traj);
   k_kpc_set_count<<<1, 1, 0, st>>>(k->map, k->count);
@@ -346,6 +371,15 @@ int vppb_kpc_trajectories_update(void* handle, void* stream) {
   if (k->n == 0) return VPPB_OK;
   k_kpc_traj<<<grid_for(k->n), 256, 0, as_stream(stream)>>>(arrays(k, k->cur), k->n, k->max_traj);
   VPPB_LAUNCH_CHECK("vppb_kpc_trajectories_update");
+  return VPPB_OK;
+}
+
+int vppb_kpc_history(void* handle, vppb_int2* velocity_dev, vppb_float2* history_dev, void* stream) {
+  VPPB_REQUIRE(handle, VPPB_E_ARG, "vppb_kpc_history: NULL container");
+  Kpc* k = static_cast<Kpc*>(handle);
+  if (k->n == 0 || (!velocity_dev && !history_dev)) return VPPB_OK;
+  k_kpc_history<<<grid_for(k->n), 256, 0, as_stream(stream)>>>(arrays(k, k->cur), k->n, k->max_traj, velocity_dev, history_dev);
+  VPPB_LAUNCH_CHECK("vppb_kpc_history");
   return VPPB_OK;
 }
 

@@ -205,3 +205,27 @@ def device_state_table(ctx, stream=None):
         return np.zeros((0, 6), dtype=np.int32)
     capi.check(capi.lib.vppb_kpc_state_table(ctx.handle, ctx._bufs["table"].ptr, stream))
     return ctx._bufs["table"].to_host(np.int32, n * 6, stream).reshape(-1, 6)
+
+
+def device_trajectories(ctx, stream=None):
+    """(vel, hist): (n, 2) int velocities and (n, max_trajectory_length, 2) float trajectory points (row, col), newest first,
+    NaN past each trajectory's length - the histories trajectories() of the host context holds."""
+    from . import capi
+    from .ops import _DeviceBuffer
+
+    n = capi.lib.vppb_kpc_size(ctx.handle)
+    if n == 0:
+        return np.zeros((0, 2), np.int32), np.zeros((0, ctx.max_traj, 2), np.float32)
+    vel, hist = _DeviceBuffer(n * 8), _DeviceBuffer(n * ctx.max_traj * 8)
+    capi.check(capi.lib.vppb_kpc_history(ctx.handle, vel.ptr, hist.ptr, stream))
+    return vel.to_host(np.int32, n * 2, stream).reshape(n, 2), hist.to_host(np.float32, n * ctx.max_traj * 2, stream).reshape(n, ctx.max_traj, 2)
+
+
+def trajectories(ctx, max_trajectory_length):
+    """(vel, hist) of a host context in the layout of device_trajectories()."""
+    n = len(ctx.pos)
+    hist = np.full((n, max_trajectory_length, 2), np.nan, np.float32)
+    for i, t in enumerate(ctx.trajectories):
+        if t.history:
+            hist[i, :len(t.history)] = t.history
+    return np.asarray(ctx.vel, np.int32).reshape(n, 2), hist
