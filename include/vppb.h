@@ -155,7 +155,8 @@ int vppb_pyrlk_prepare(const vppb_img* i1, const vppb_img* i2, const vppb_img* p
 enum { VPPB_FAST_REFERENCE_RING = 0, VPPB_FAST_TRUE_RING = 1 };
 enum { VPPB_FAST_ALL = 0, VPPB_FAST_LOCAL_MAXIMA = 1, VPPB_FAST_BLOCKWISE = 2 };
 /* Workspace bytes needed by vppb_fast9_u8 for an nrows x ncols image (block_size: the blockwise cell side, or <= 0
- * for a workspace that is large enough for every mode and block size). */
+ * for a workspace that is large enough for every mode and block size).  The workspace must be 256-byte aligned (any vppb_alloc or
+ * cudaMalloc pointer is): vppb_fast9_u8, _async and vppb_fast9_blockwise_rank_u8 return VPPB_E_ARG for any other pointer. */
 int64_t vppb_fast9_workspace_bytes(int32_t nrows, int32_t ncols, int32_t block_size);
 /* fast9(A, th, [_local_maxima|_blockwise, _block_size=, _mask=, _scores=]).
  * mask may be NULL (== 0xFF everywhere).  kps_out (device, capacity records) receives the
@@ -181,7 +182,8 @@ int vppb_fast9_scores(const vppb_img* img, int32_t th, const vppb_int2* kps, int
 /* fast_detector9_blockwise_rank (fast.hpp:801-886, on fast_detector9_maxima2 fast.hpp:710-740): up to max_points (<= 16) ranked
  * keypoints per block_size x block_size block - the strict 3x3 maxima of the RAW score image (0 where nothing was detected), kept by
  * the reference's table rule and sorted by decreasing score.  kps3_out (device int32 triples): (row, col, rank), blocks in raster
- * order, ranks ascending; scores_out (device, may be NULL): raw scores; count_out (host).  Synchronises the stream. */
+ * order, ranks ascending; scores_out (device, may be NULL): raw scores; count_out (host).  Synchronises the stream.  Workspace:
+ * 256-byte aligned (VPPB_E_ARG otherwise). */
 int64_t vppb_fast9_rank_workspace_bytes(int32_t nrows, int32_t ncols, int32_t block_size, int32_t max_points);
 int vppb_fast9_blockwise_rank_u8(const vppb_img* img, int32_t th, const vppb_img* mask, int32_t block_size, int32_t max_points,
                                  int32_t ring, void* workspace, int64_t workspace_bytes, int32_t* kps3_out, int32_t* scores_out,
@@ -193,7 +195,8 @@ int vppb_fast9_blockwise_rank_u8(const vppb_img* img, int32_t th, const vppb_img
 int vppb_lbp_u8(const vppb_img* in, const vppb_img* out, void* stream);
 /* local_maxima_filter(A, nbh_size) (fast.hpp:555-575; nbh_size is ignored there too): IN PLACE, a pixel that is not strictly greater
  * than its 8 neighbours becomes 0 - with the reference's serial raster-order semantics (the neighbours above and to the left have
- * already been filtered).  unsigned char or int pixels, border >= 1 (read, never written).  One cooperative launch. */
+ * already been filtered).  unsigned char or int pixels, border >= 1 (read, never written).  One cooperative launch.  The workspace
+ * (at least vppb_local_maxima_filter_workspace_bytes bytes) must be 256-byte aligned (VPPB_E_ARG otherwise). */
 int64_t vppb_local_maxima_filter_workspace_bytes(int32_t nrows, int32_t ncols, int32_t elem_bytes);
 int vppb_local_maxima_filter(const vppb_img* img, void* workspace, int64_t workspace_bytes, void* stream);
 
@@ -204,7 +207,8 @@ int vppb_local_maxima_filter(const vppb_img* img, void* workspace, int64_t works
  * domain pixel the mask distance to the nearest zero of `in`, capped at B.  `in`: unsigned char or int pixels compared with 0, its
  * border is not read; `out`: int, same domain, border >= 1 (>= 2 for d5-7-11: VPPB_E_BORDER), no memory shared with `in` (VPPB_E_ARG).
  * Pitch padding is never written.  A fixed number of launches per mask, no host synchronisation; `workspace` is device memory of at
- * least vppb_distance_transform_workspace_bytes bytes, used until the work queued on `stream` completes. */
+ * least vppb_distance_transform_workspace_bytes bytes, 8-byte aligned (VPPB_E_ARG otherwise, unless that size is 0), used until the
+ * work queued on `stream` completes. */
 enum { VPPB_DT_D4 = 0, VPPB_DT_D8 = 1, VPPB_DT_D3_4 = 2, VPPB_DT_D5_7_11 = 3 };
 int64_t vppb_distance_transform_workspace_bytes(int32_t nrows, int32_t ncols, int32_t kind);
 int vppb_distance_transform(const vppb_img* in, const vppb_img* out, int32_t kind, void* workspace, int64_t workspace_bytes, void* stream);
@@ -280,6 +284,7 @@ typedef struct vppb_sdof_params {
   int32_t propagation;  /* number of neighbour-propagation sweeps per scale, >= 0 (even sweeps backward, odd forward) */
   int32_t patchsize;    /* cell side, >= 1 */
 } vppb_sdof_params;
+/* Workspace bytes of vppb_sdof_u8; the workspace must be 256-byte aligned (VPPB_E_ARG otherwise). */
 int64_t vppb_sdof_workspace_bytes(int32_t nrows, int32_t ncols, const vppb_sdof_params* params);
 /* pyr1 / pyr2: `nscales` u8 pyramid levels of the two frames (pyramid2d<uchar>(img, nscales, 2, _border >= winsize/2),
  * borders mirror-filled).  kps: n device (row, col) records.  For keypoint i, out_valid[i] tells whether the reference

@@ -676,6 +676,7 @@ static int fast9_core(const vppb_img* img, int32_t th, const vppb_img* mask, int
   // the reference ignores block_size outside the blockwise mode: so does the workspace rule
   FastWs ws = fast_ws_layout(workspace, img->nrows, img->ncols, mode == VPPB_FAST_BLOCKWISE && !rank ? block_size : (1 << 30));
   const long long need = ws.bytes + (rank ? fast_rank_bytes(img->nrows, img->ncols, block_size, rank->maxp) : 0);
+  VPPB_REQUIRE((uintptr_t)workspace % 256 == 0, VPPB_E_ARG, "%s: workspace not 256-byte aligned", name);
   VPPB_REQUIRE(workspace_bytes >= need, VPPB_E_ARG, "%s: workspace %lld < %lld bytes", name, (long long)workspace_bytes, need);
   cudaStream_t st = as_stream(stream);
   const int wpr = (img->ncols + 31) / 32;

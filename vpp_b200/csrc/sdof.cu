@@ -668,6 +668,7 @@ int vppb_sdof_u8(const vppb_img* pyr1, const vppb_img* pyr2, const vppb_sdof_par
   VPPB_REQUIRE(n == 0 || (kps && out_pos && out_dist && out_valid), VPPB_E_ARG, "vppb_sdof_u8: NULL keypoint/output array");
   VPPB_REQUIRE(p->nscales >= 1 && p->nscales <= 8 && p->min_scale >= 0 && p->min_scale < p->nscales && p->patchsize >= 1 && p->winsize >= 1 &&
                    p->winsize <= 15 && p->propagation >= 0, VPPB_E_ARG, "vppb_sdof_u8: parameters out of range");
+  VPPB_REQUIRE((uintptr_t)workspace % 256 == 0, VPPB_E_ARG, "vppb_sdof_u8: workspace not 256-byte aligned");
   VPPB_REQUIRE(workspace_bytes >= vppb_sdof_workspace_bytes(pyr1[0].nrows, pyr1[0].ncols, p), VPPB_E_ARG, "vppb_sdof_u8: workspace too small");
   cudaStream_t st = as_stream(stream);
   SdofLevel L[8];

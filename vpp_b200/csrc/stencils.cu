@@ -169,6 +169,7 @@ int vppb_local_maxima_filter(const vppb_img* img, void* workspace, int64_t works
   VPPB_REQUIRE(img->elem_bytes == 1 || img->elem_bytes == 4, VPPB_E_ARG, "vppb_local_maxima_filter: unsigned char or int pixels expected");
   VPPB_REQUIRE(img->border >= 1, VPPB_E_BORDER, "vppb_local_maxima_filter: the image needs a border of 1 pixel");
   const int64_t need = vppb_local_maxima_filter_workspace_bytes(img->nrows, img->ncols, img->elem_bytes);
+  VPPB_REQUIRE((uintptr_t)workspace % 256 == 0, VPPB_E_ARG, "vppb_local_maxima_filter: workspace not 256-byte aligned");
   VPPB_REQUIRE(workspace_bytes >= need, VPPB_E_ARG, "vppb_local_maxima_filter: workspace %lld < %lld bytes", (long long)workspace_bytes, (long long)need);
   if (img->nrows == 0 || img->ncols == 0) return VPPB_OK;
   cudaStream_t st = as_stream(stream);
@@ -427,6 +428,8 @@ int vppb_distance_transform(const vppb_img* in, const vppb_img* out, int32_t kin
   VPPB_REQUIRE(!(in->alloc && in->alloc == out->alloc) && (ihi <= olo || ohi <= ilo), VPPB_E_ARG,
                "vppb_distance_transform: the input and the output share memory");
   const int64_t need = dt_ws_bytes(in->nrows, in->ncols, m);
+  // the workspace holds int2 segment summaries: 8-byte alignment is what they need (a host or malloc'ed block qualifies)
+  VPPB_REQUIRE(need == 0 || (uintptr_t)workspace % 8 == 0, VPPB_E_ARG, "vppb_distance_transform: workspace not 8-byte aligned");
   VPPB_REQUIRE(need == 0 || (workspace && workspace_bytes >= need), VPPB_E_ARG, "vppb_distance_transform: workspace %lld < %lld bytes",
                (long long)workspace_bytes, (long long)need);
 
